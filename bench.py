@@ -1,4 +1,4 @@
-"""bench.py — headline benchmark of the FateZero hot path on B200.
+"""bench.py — headline benchmark of the FateZero hot path on H100.
 
 metric  : edited frames/sec = F / (T_inversion + T_edit) for one 512x512x8-frame clip, 50 DDIM steps, one target prompt
           (BASELINE.json / SURVEY.md §8(d)); one "step" of this script = ONE full clip edit (50 inversion UNet forwards with the
@@ -6,11 +6,13 @@ metric  : edited frames/sec = F / (T_inversion + T_edit) for one 512x512x8-frame
 value   : inputs already resident in HBM when the timed region starts.
 e2e     : the same edit through the reference-facing API with HOST buffers: per step the clean latents are copied from pinned host
           memory and the edited latents are read back to the host inside the timed region.
-roofline: the dominant kernel is the tcgen05 tap-GEMM (convs + linears + temporal LoRA, 86% of the FLOPs): algorithmic FLOPs of all its
-          launches in one clip edit / the sum of their CUDA-event durations (instrumented extra pass), against the measured bf16 peak.
+roofline: the dominant kernel is the wgmma tap-GEMM (convs + linears + temporal LoRA, 86% of the FLOPs): algorithmic FLOPs of all its
+          launches in one clip edit / the sum of their CUDA-event durations (instrumented extra pass), against the dense fp16 peak.
 st_attn : ST-attn TFLOPS = sum over the spatio-temporal attention launches of a clip of 4*BF*heads*S*T*d / sum of their CUDA-event durations.
 vae     : the VAE bracket (encode + decode of the clip's frames on the tap-GEMM), reported next to the metric, not inside it.
-Launch:  python bench.py [--gpus N --steps K --warmup W] [--config style|attribute|long24|shape768]
+outputs : --dump-outputs DIR writes what the timed path returned in its last timed step (the edited latents, float32) as
+          DIR/<name>.npy; weights and inputs are seeded, so two builds run with the same arguments can be compared output for output.
+Launch:  python bench.py [--gpus N --steps K --warmup W] [--config style|attribute|long24|shape768] [--dump-outputs DIR]
          N>1 under torch.distributed.run, one rank per GPU: the frames of ONE clip are split over the ranks with the same weights as N=1
          ("strong" scaling; exchanges = peer-memory push/flag kernels, DESIGN.md §6); --shard clips = independent clips per rank (replicas)
          python bench.py --impl reference ...   (CPU arm: the oracle port of the reference on the host cores, one full-frame step pair per step)
@@ -51,7 +53,7 @@ CONFIGS = {
         tgt="watercolor painting of " + SRC,
         p2p=dict(is_replace_controller=False, cross_replace_steps={"default_": 0.8}, self_replace_steps=0.8,
                  eq_params={"words": ["watercolor"], "values": [10, 10]}),
-        workload="long clip: 512x512x24f, 50 DDIM steps, Refine+Reweight, frames sharded over the GPUs (109 GiB of maps per clip)"),
+        workload="long clip: 512x512x24f, 50 DDIM steps, Refine+Reweight, frames sharded over the GPUs (109 GiB of maps per clip: >= 2 GPUs of 80 GB)"),
     "shape768": dict(  # config/shape/jeep_posche.yaml p2p_config[1] semantics: default [-1,'first'] K/V frames, ST-attn at every resolution
         frames=16, size=96, model_config=dict(lora=160),
         tgt="a Porsche car driving down a curvy road in the countryside",
@@ -74,11 +76,12 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return dict(bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, hbm_gbs=6650.0), "fallback"
+        # NVIDIA H100 SXM data sheet (700 W): dense fp16 / bf16 tensor rate and HBM3 bandwidth, not measured here
+        return dict(bf16_tflops=989.0, hbm_gbs=3350.0), "H100 SXM data sheet"
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling (nvidia-smi, read-only queries)
 # ------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -212,6 +215,11 @@ def instrument(pipe, x0_dev, emb_src):
                                                         timed(ops.attention, on_attn))
     mode = pipe.graph_mode
     pipe.graph_mode = "off"  # the instrumented pass needs the Python-level launches (a graph replay does not pass through ops.*)
+    # the eager clip allocates a map cache of its own (36 GiB at 512x512x8f): free the captured loops' pools and cache first, an 80 GB
+    # card does not hold both
+    pipe.release_graphs()
+    pipe.store_controller.reset()
+    torch.cuda.empty_cache()
     try:
         edit_clip(pipe, x0_dev, emb_src)
         torch.cuda.synchronize()
@@ -286,6 +294,10 @@ def run_gpu(args):
     shard_frames = world > 1 and args.shard == "frames"
     if shard_frames and FRAMES % world:
         raise SystemExit(f"{FRAMES} frames do not split over {world} GPUs")
+    if CFG["name"] == "long24" and not shard_frames:
+        # 109 GiB of attention maps per clip: more than one 80 GB GPU holds, 54.5 GiB per GPU with the frames over two
+        raise SystemExit("--config long24 needs the frames of the clip sharded over >= 2 GPUs: torchrun --nproc-per-node 2 bench.py --gpus 2 "
+                         "--config long24")
     pipe = build_pipe(device)
     if shard_frames:
         from fatezero_b200 import dist as fzdist
@@ -294,8 +306,8 @@ def run_gpu(args):
         x0_host = fzdist.frame_slice(x_full, rank, world).pin_memory()
     else:
         x0_host = (synth.synth_latents(FRAMES, SIZE, SIZE, seed=1 + rank) * 0.5).pin_memory()
-    if args.graphs == "off" or (CFG["name"] == "long24" and world < 2):
-        pipe.graph_mode = "off"  # 24 frames on one GPU: 109 GiB of maps, no room for an eager copy next to the graph pool
+    if args.graphs == "off":
+        pipe.graph_mode = "off"
     out_host = torch.empty_like(x0_host).pin_memory()
     x0_dev = x0_host.to(device)
     emb_src = pipe._encode_prompt(SRC, device, 1, True, None)
@@ -324,8 +336,10 @@ def run_gpu(args):
             ms = float(t.item())
         return ms
 
+    last = {}
+
     def step_resident():
-        edit_clip(pipe, x0_dev, emb_src)
+        last["edited_latents"] = edit_clip(pipe, x0_dev, emb_src)
 
     def step_e2e():
         xd = x0_host.to(device, non_blocking=True)
@@ -344,6 +358,11 @@ def run_gpu(args):
     host_ms.clear()
     ms = timed(step_resident, args.steps)
     launches = _lib.kernel_launches - launches0
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in last.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.detach().float().cpu().numpy())
     clocks = sampler.stop() if rank == 0 else None
     ms_e2e = timed(step_e2e, args.steps)
     frames_total = FRAMES * (1 if (shard_frames or world == 1) else world) * args.steps
@@ -359,20 +378,11 @@ def run_gpu(args):
             inst = instrument(pipe, x0_dev, emb_src)
     if rank == 0 and inst is not None:
         flops, secs, n_launch, abytes = inst["gemm"]
-        peak = float(pk.get("bf16_tflops_sustained", pk.get("bf16_tflops", 1400.0)))
+        peak = float(pk.get("bf16_tflops_sustained", pk.get("bf16_tflops", 989.0)))
         ach = flops / secs / 1e12
-        # DRAM bytes per tap-GEMM launch from the committed ncu capture of one step pair of THIS round, if present
-        traffic = traffic_src = None
-        for cand in ("r02_tapgemm_traffic.json",):
-            try:
-                tj = json.load(open(os.path.join(ROOT, "profiles", cand)))
-                traffic, traffic_src = round(tj["tapgemm_dram_bytes_per_launch"]), f"profiles/{cand}: {tj.get('how', 'ncu dram__bytes_read+write per launch')}"
-                break
-            except Exception:  # noqa: BLE001
-                pass
-        roof = dict(kernel="tapgemm_kernel (conv3x3 / linear / temporal-LoRA, tcgen05)", bound="tensor", achieved=round(ach, 1), peak=peak,
-                    unit="TFLOP/s", frac=round(ach / peak, 4), traffic=traffic, traffic_source=traffic_src,
-                    algorithmic_bytes_per_launch=round(abytes / max(n_launch, 1)), peak_source=f"{pk_kind} sustained bf16 (MEASURED_PEAKS.json)",
+        roof = dict(kernel="tapgemm_kernel (conv3x3 / linear / temporal-LoRA, wgmma)", bound="tensor", achieved=round(ach, 1), peak=peak,
+                    unit="TFLOP/s", frac=round(ach / peak, 4),
+                    algorithmic_bytes_per_launch=round(abytes / max(n_launch, 1)), peak_source=f"{pk_kind} dense fp16/bf16",
                     launches_per_clip=n_launch, algorithmic_tflop_per_clip=round(flops / 1e12, 1),
                     kernel_seconds_per_clip=round(secs, 4), share_of_step=round(secs / (ms / 1e3 / args.steps), 3),
                     how="CUDA events around every launch of an extra eager clip (per rank: this rank's frames)")
@@ -396,7 +406,7 @@ def run_gpu(args):
                     data="synthetic",
                     config=dict(workload=CFG["workload"], name=CFG["name"], frames=FRAMES, latent=f"{SIZE}x{SIZE}", ddim_steps=DDIM_STEPS,
                                 model_config=CFG["model_config"], parallelism=par, cuda_graphs=pipe.graph_mode,
-                                l2="working set (map cache of the clip + activations) far exceeds the 126 MB L2; no explicit flush"),
+                                l2="working set (map cache of the clip + activations) far exceeds the 50 MB L2; no explicit flush"),
                     clocks=clocks, e2e=dict(value=round(e2e_value, 4), unit="frames/s", h2d_bytes_per_step=x0_host.numel() * 4,
                                             d2h_bytes_per_step=out_host.numel() * 4),
                     gpu_launches=int(launches), st_attn_tflops=st, vae=vae_line, roofline=roof,
@@ -495,6 +505,8 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the edited latents of the last timed step as DIR/<name>.npy (float32) for output-for-output comparisons")
     ap.add_argument("--config", default="style", choices=sorted(CONFIGS), help="BASELINE.json configs #2..#5 (default: the metric's own)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-instrument", action="store_true", help="skip the extra instrumented clip (roofline / ST-attn TFLOPS)")

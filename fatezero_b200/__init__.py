@@ -1,4 +1,4 @@
-"""fatezero_b200 — B200-native (sm_100a) implementation of FateZero's DDIM-inversion + attention-fused denoising hot path.
+"""fatezero_b200 — H100-native (sm_90a) implementation of FateZero's DDIM-inversion + attention-fused denoising hot path.
 
     from fatezero_b200 import UNetPseudo3DConditionModel, P2pDDIMSpatioTemporalPipeline, DDIMScheduler
     (or the reference's own import paths through the `video_diffusion` alias package)

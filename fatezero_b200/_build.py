@@ -1,4 +1,4 @@
-"""Build libfatezero_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libfatezero_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfatezero_b200.so")
 SOURCES = ["fz_capi.cu", "fz_gemm.cu", "fz_elem.cu", "fz_attn.cu", "fz_p2p.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "--use_fast_math" if False else "-DFZ_NO_FAST_MATH"]
 
 
@@ -52,7 +53,7 @@ def _build(lib: str, objdir: str, extra_flags, verbose: bool) -> str:
         out, _ = p.communicate()
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed on {src}:\n{out.decode()}")
-    cmd = [_nvcc(), "-shared", "-o", lib, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [_nvcc(), "-shared", "-o", lib, *objs, *ARCH]
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.check_call(cmd)

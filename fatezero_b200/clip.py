@@ -1,4 +1,4 @@
-"""CLIP text encoder on the sm_100a kernels (SURVEY.md §8(f) rank 4).  The reference encodes prompts with transformers' CLIPTextModel
+"""CLIP text encoder on the sm_90a kernels (SURVEY.md §8(f) rank 4).  The reference encodes prompts with transformers' CLIPTextModel
 (`pipelines/stable_diffusion.py:230,279`: `self.text_encoder(ids, attention_mask=...)[0]`); `ClipTextEngine` executes the same pre-LN
 transformer (token + position embedding, 12 x {LN, causal self-attention, LN, quick_gelu MLP}, final LN) with fz_layernorm / fz_gemm /
 fz_attention (causal = 1) / fz_quick_gelu: fp16 storage, fp32 accumulation, fp32 output.  Weights are read from a CLIPTextModel-shaped

@@ -1,4 +1,4 @@
-// fz_attn.cu — fused attention for the FateZero hot path (sm_100a: TMA + tcgen05 + TMEM).
+// fz_attn.cu — fused attention for the FateZero hot path (sm_90a: TMA + wgmma).
 //
 // One kernel computes  O = f(softmax(scale * Q K^T)) V  for
 //   * the spatio-temporal self-attention (K/V of 0..n frames selected per query frame:
@@ -11,14 +11,17 @@
 //              (attention_util.py:80-92 without mask)
 //   BLEND      edit, self-attention with a per-(frame,pixel) mask: rows with mask==0 take the cached row (:86-88)
 //   CROSSEDIT  edit, cross-attention: Refine gather / Replace 77x77 / Reweight / alpha-lerp in registers (:130-131,213-253,282-286)
-// Two passes over the keys (max[/sum] first, then probabilities): the normalised fp16 P the reference stores and multiplies is
-// reproduced exactly at its rounding point; rows that are neither stored nor edited use the cheaper "max only" first pass and
-// normalise O at the end.
+// Hooked rows take two passes over the keys (max and sum first, then probabilities): the normalised fp16 P the reference stores and
+// multiplies is reproduced exactly at its rounding point.  Rows that are neither stored nor edited take ONE pass with a running reference
+// maximum (online softmax: p = exp2(s c - m_ref c) rounded to fp16 for PV, fp32 row sum l, O / l at the end; m_ref is raised, and O, l
+// rescaled, only when a key block exceeds it by more than 2^8, so the rescale is rare and p stays far inside fp16 range).
 //
-// CTA = 128 query rows of one (frame, head); 10 warps: 0 = TMA producer, 1 = MMA issuer, 2..9 = two softmax / epilogue warpgroups
-// (1 row per thread each; warpgroup w handles key blocks b with b % 2 == w so two warps per scheduler hide MUFU / TMEM latencies).
-// TMEM: S double buffer (2 x 128 cols) + O (<= 192 cols).  smem: Q tile, a ring of K / V^T atoms, P double buffer (+ base P).
+// CTA = 128 query rows of one (frame, head); 9 warps: 0-7 = two consumer warpgroups (warpgroup w owns query rows [64 w, 64 w + 64):
+// it issues the wgmma of S = Q K^T and O += P V for them, holds S and O in registers and runs the softmax and the controller hook),
+// 8 = TMA producer.  Pipeline granularity = one ATOM of 64 keys.  smem: Q tile, a ring of K chunks / V^T atoms shared by both
+// warpgroups, two P buffers per warpgroup (64 rows x 64 keys, swizzled) and two cached-P ("base") buffers for REPLACE / BLEND.
 #include "fz_common.cuh"
+#include "fz_wgmma.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -30,18 +33,19 @@ namespace fz {
 constexpr int kMaxSlots = 4;
 constexpr int kMaxBF = 64;
 constexpr int kAtomBytes = 128 * 128;  // 128 rows x 64 fp16
+constexpr int kHalfAtom = 64 * 128;    // one warpgroup's 64 rows
+constexpr int kMaxStages = 12;
 
 struct AttnParams {
   CUtensorMap tmQ;      // (d, heads, S_q, BF)                 box (64, 1, 128, 1)
   CUtensorMap tmK;      // (d, heads, keys_per_slot, SRC)      box (64, 1, 64, 1)
-  CUtensorMap tmVt;     // (keys_ld, d, heads, SRC)            box (64, d_pad, 1, 1)
-  CUtensorMap tmK2;     // tmK with box (64, 1, 128, 1): 128-key tiles of the plain kernel
-  CUtensorMap tmStore;  // (keys_ld_cache, slots, S_q, heads, Fc) box (64, 1, 128, 1, 1)   cache slab written (STORE)
+  CUtensorMap tmVt;     // (keys_ld, d, heads, SRC)            box (64, 64 nd, 1, 1)
+  CUtensorMap tmStore;  // (keys_ld_cache, slots, S_q, heads, Fc) box (64, 1, 64, 1, 1)   cache slab written (STORE)
   CUtensorMap tmBase;   // same geometry, cache slab read (REPLACE / BLEND)
   int S_q;              // queries per (frame, head)
   int keys_per_slot;    // S for self-attention, 77 for cross
   int n_slots;          // key/value frames per query frame (self: 1..4, cross: 1)
-  int d, d_pad, nd;     // head dim, padded to 16, number of 64-wide chunks
+  int d, nd;            // head dim, number of 64-wide chunks
   int heads, F, BF;
   int ring_stages, ring_stage_bytes;
   float scale_log2;     // scale * log2(e)
@@ -57,8 +61,8 @@ struct AttnParams {
   const float* mask;    // BLEND: [Fc, S_q] 1 = keep current row, 0 = take cached row
   __half* out;          // [BF*S_q, ldo], this head's columns start at head*d
   long long ldo;
-  long long* dbg;       // optional [32] cycle counters written by CTA (0,0,0) (profiling aid)
-  int causal;           // key n visible to query s only if n <= s (kMasked instantiation only)
+  int causal;           // key n visible to query s only if n <= s
+  int masked;           // keys_per_slot % 64 != 0 or causal: scores outside the valid keys are set to -inf
 };
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
@@ -70,41 +74,14 @@ __device__ __forceinline__ float ex2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// 2^y for y <= ~8 on the FMA / ALU pipes (no MUFU): floor via a round-down magic-number add, degree-4 minimax polynomial for the
-// fraction (max relative error 2.7e-6, far below the fp16 rounding of the probability), exponent inserted with integer arithmetic.
-// The plain attention kernel is MUFU-bound (16 ex2 / clk / SM, tools/micro/exp_rate.cu), so a quarter of its exponentials take this
-// path (measured: 20.5 exp / clk / SM for the 3:1 mix).
-__device__ __forceinline__ float ex2_poly(float y) {
-  y = fmaxf(y, -125.f);                         // also maps -inf (masked keys) to 2^-125, which fp16 rounds to zero
-  const float yr = __fadd_rd(y, 12582912.f);    // 1.5 * 2^23 + floor(y)
-  const float fl = yr - 12582912.f;
-  const float f = y - fl;                       // [0, 1)
-  float p = fmaf(0.013534133322536945f, f, 0.05201148986816406f);
-  p = fmaf(p, f, 0.24144276976585388f);
-  p = fmaf(p, f, 0.6930038332939148f);
-  p = fmaf(p, f, 1.0000026226043701f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(yr) << 23));
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-
-// Optional in-kernel cycle accounting (compile with -DFZ_ATTN_PROFILE): adds clock reads around the waits of CTA (0,0,0).
-#ifdef FZ_ATTN_PROFILE
-#define FZ_TIMED(slot, stmt)                       \
-  do {                                             \
-    if (dbg_on) {                                  \
-      const long long _t0 = clock64();             \
-      stmt;                                        \
-      dbg_acc[slot] += clock64() - _t0;            \
-    } else {                                       \
-      stmt;                                        \
-    }                                              \
-  } while (0)
-#else
-#define FZ_TIMED(slot, stmt) \
-  do {                       \
-    stmt;                    \
-  } while (0)
-#endif
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 
 struct AtomInfo {
   int slot, k0, valid;
@@ -122,13 +99,23 @@ __device__ __forceinline__ AtomInfo atom_info(const AttnParams& p, int atoms_per
   return a;
 }
 
-// Pipeline granularity = one ATOM of 64 keys.  TMEM: 4 S buffers of 64 columns ([0,256)) + O at column 256.  smem: 4 P buffers
-// (128 rows x 64 keys, swizzled) + 2 cached-P ("base") buffers for BLEND.  Softmax warpgroup w owns the atoms with (A & 1) == w,
-// hence S buffers {w, w+2} (mod pass offset), P buffers {w, w+2} and base buffer w: every mbarrier is waited on by one agent in
-// program order, so parity waits can never run two phases ahead.
-// kMasked: keys_per_slot is not a multiple of 64 (text cross-attention: 77 keys); the un-masked instantiation has no masking code in its loops.
-template <bool kMasked>
-__global__ void __launch_bounds__(320, 1) attn_kernel(const __grid_constant__ AttnParams p) {
+// O[64 x 64 NCH] (+)= P[64 x 64 keys] V[64 keys x 64 NCH]: the V^T atom holds 64 NCH rows (TMA zero-fills the rows beyond d), so every
+// chunk is one fixed-shape wgmma and the issue sequence has no data-dependent branch (which would serialise the asynchronous MMAs).
+template <int NCH>
+__device__ __forceinline__ void pv_mma(float (&o)[32 * NCH], uint64_t da, uint64_t db, uint32_t accumulate) {
+#pragma unroll
+  for (int ch = 0; ch < NCH; ++ch) {
+    const uint64_t dbc = db + static_cast<uint32_t>((ch * 64 * 128) >> 4);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_f16<64>(o + 32 * ch, da + 2 * k, dbc + 2 * k, (accumulate | k) ? 1u : 0u);
+  }
+}
+
+constexpr float kRescaleThreshold = 8.0f;  // log2 units: un-hooked rows raise their reference maximum only past 2^8 (fp16 P stays finite)
+
+// NCH = number of 64-wide chunks of the head dim (1..3): sizes the O accumulator (32 NCH registers per thread).
+template <int NCH>
+__global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -145,21 +132,15 @@ __global__ void __launch_bounds__(320, 1) attn_kernel(const __grid_constant__ At
 
   uint8_t* s_q = smem;
   uint8_t* s_ring = s_q + p.nd * kAtomBytes;
-  uint8_t* s_p = s_ring + p.ring_stages * p.ring_stage_bytes;  // 4 x 16 KiB
-  uint8_t* s_pbase = s_p + 4 * kAtomBytes;                     // 2 x 16 KiB (BLEND only)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_pbase + (p.row_mode == FZ_ATTN_BLEND ? 2 * kAtomBytes : 0));
-  uint64_t* ring_full = bars;        // [12]
-  uint64_t* ring_empty = bars + 12;  // [12]
-  uint64_t* q_full = bars + 24;
-  uint64_t* s_full = bars + 25;      // [4]
-  uint64_t* s_empty = bars + 29;     // [4]
-  uint64_t* p_full = bars + 33;      // [4]
-  uint64_t* p_empty = bars + 37;     // [4]
-  uint64_t* o_full = bars + 41;
-  uint64_t* base_full = bars + 42;   // [2]
-  uint64_t* base_empty = bars + 44;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 46);
-  float* xchg = reinterpret_cast<float*>(bars + 48);  // [2 warpgroups][128 rows][2]
+  uint8_t* s_p = s_ring + p.ring_stages * p.ring_stage_bytes;  // [warpgroup][2] x 8 KiB
+  uint8_t* s_base = s_p + 4 * kHalfAtom;                       // 2 x 16 KiB (REPLACE / BLEND only)
+  const bool has_base = p.row_mode == FZ_ATTN_REPLACE || p.row_mode == FZ_ATTN_BLEND;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_base + (has_base ? 2 * kAtomBytes : 0));
+  uint64_t* ring_full = bars;                   // [kMaxStages]
+  uint64_t* ring_empty = bars + kMaxStages;     // [kMaxStages]
+  uint64_t* q_full = bars + 2 * kMaxStages;
+  uint64_t* base_full = q_full + 1;             // [2]
+  uint64_t* base_empty = base_full + 2;         // [2]
 
   const int atoms_per_slot = (p.keys_per_slot + 63) / 64;
   const int n_atoms = atoms_per_slot * p.n_slots;
@@ -168,403 +149,244 @@ __global__ void __launch_bounds__(320, 1) attn_kernel(const __grid_constant__ At
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmVt);
-    for (int s = 0; s < 12; ++s) {
+    for (int s = 0; s < p.ring_stages; ++s) {
       mbar_init(&ring_full[s], 1);
-      mbar_init(&ring_empty[s], 1);
+      mbar_init(&ring_empty[s], 8);  // every consumer warp releases every stage
     }
     mbar_init(q_full, 1);
-    for (int b = 0; b < 4; ++b) {
-      mbar_init(&s_full[b], 1);
-      mbar_init(&s_empty[b], 4);
-      mbar_init(&p_full[b], 1);
-      mbar_init(&p_empty[b], 1);
-    }
-    mbar_init(o_full, 1);
     for (int b = 0; b < 2; ++b) {
       mbar_init(&base_full[b], 1);
-      mbar_init(&base_empty[b], 4);
+      mbar_init(&base_empty[b], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 9) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();  // prologue above overlaps the previous kernel's tail (programmatic dependent launch)
-  const uint32_t tmem_o = tmem_base + 256;
-#ifdef FZ_ATTN_PROFILE
-  const bool dbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;  // warp-uniform
-#else
-  constexpr bool dbg_on = false;
-#endif
-  long long dbg_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  const long long dbg_t0 = clock64();
 
-  // Warp roles: 0..7 softmax (two warpgroups), 8 = TMA producer, 9 = MMA issuer.  The issue arbiter favours higher warp ids, and the
-  // MMA warp gates everything downstream, so it gets the highest id (as warp 1 it was starved by the softmax warps of its scheduler).
   if (warp == 8) {
     // =========================================== TMA producer ===========================================
-    if (elect_one()) {
+    if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       auto advance = [&]() { if (++stage == p.ring_stages) { stage = 0; phase ^= 1; } };
-      // K chunks of an atom PAIR are interleaved (A.c0, A+1.c0, A.c1, ...) to match the MMA warp's interleaved issue order
-      auto load_k_pair = [&](int A0) {
-        const int n = min(2, n_atoms - A0);
-        const AtomInfo a0 = atom_info(p, atoms_per_slot, A0);
-        const AtomInfo a1 = atom_info(p, atoms_per_slot, min(A0 + 1, n_atoms - 1));
+      auto load_k = [&](int A) {
+        const AtomInfo ai = atom_info(p, atoms_per_slot, A);
         for (int c = 0; c < p.nd; ++c) {
-          for (int j = 0; j < n; ++j) {
-            const AtomInfo& ai = j ? a1 : a0;
-            mbar_wait(&ring_empty[stage], phase ^ 1);
-            mbar_expect_tx(&ring_full[stage], 64 * 128);
-            tma_load_4d(s_ring + stage * p.ring_stage_bytes, &p.tmK, &ring_full[stage], c * 64, head, ai.k0, p.src_index[ai.slot][bf]);
-            advance();
-          }
+          mbar_wait(&ring_empty[stage], phase ^ 1);
+          mbar_expect_tx(&ring_full[stage], 64 * 128);
+          tma_load_4d(s_ring + stage * p.ring_stage_bytes, &p.tmK, &ring_full[stage], c * 64, head, ai.k0, p.src_index[ai.slot][bf]);
+          advance();
         }
       };
       auto load_v = [&](int A) {
         const AtomInfo ai = atom_info(p, atoms_per_slot, A);
         mbar_wait(&ring_empty[stage], phase ^ 1);
-        mbar_expect_tx(&ring_full[stage], p.d_pad * 128);
+        mbar_expect_tx(&ring_full[stage], NCH * 64 * 128);
         tma_load_4d(s_ring + stage * p.ring_stage_bytes, &p.tmVt, &ring_full[stage], ai.k0, 0, head, p.src_index[ai.slot][bf]);
         advance();
       };
-      auto load_base = [&](int A, uint8_t* dst, uint64_t* bar) {
+      auto load_base = [&](int A) {
         const AtomInfo ai = atom_info(p, atoms_per_slot, A);
-        mbar_expect_tx(bar, kAtomBytes);
-        tma_load_5d(dst, &p.tmBase, bar, ai.k0, ai.slot, q0, head, fc);
+        const int b = A & 1;
+        mbar_wait(&base_empty[b], ((A >> 1) & 1) ^ 1);
+        mbar_expect_tx(&base_full[b], kAtomBytes);
+        for (int h = 0; h < 2; ++h)
+          tma_load_5d(s_base + b * kAtomBytes + h * kHalfAtom, &p.tmBase, &base_full[b], ai.k0, ai.slot, q0 + 64 * h, head, fc);
       };
       if (!replace) {
         mbar_expect_tx(q_full, p.nd * kAtomBytes);
         for (int c = 0; c < p.nd; ++c) tma_load_4d(s_q + c * kAtomBytes, &p.tmQ, q_full, c * 64, head, q0, bf);
-        for (int A = 0; A < n_atoms; A += 2) load_k_pair(A);  // pass 1
-        load_k_pair(0);                                        // pass 2: one pair of S tiles of look-ahead
-        for (int A = 0; A < n_atoms; A += 2) {
-          if (A + 2 < n_atoms) load_k_pair(A + 2);
-          const int n = min(2, n_atoms - A);
-          if (blend) {
-            for (int j = 0; j < n; ++j) {
-              const int w = (A + j) & 1;
-              mbar_wait(&base_empty[w], (((A + j) >> 1) & 1) ^ 1);
-              load_base(A + j, s_pbase + w * kAtomBytes, &base_full[w]);
-            }
-          }
-          for (int j = 0; j < n; ++j) load_v(A + j);
+        if (exact)
+          for (int A = 0; A < n_atoms; ++A) load_k(A);  // pass 1
+        for (int A = 0; A < n_atoms; ++A) {             // pass 2 (the only pass of un-hooked rows)
+          load_k(A);
+          if (blend) load_base(A);
+          load_v(A);
         }
       } else {
-        for (int A = 0; A < n_atoms; A += 2) {
-          const int n = min(2, n_atoms - A);
-          for (int j = 0; j < n; ++j) {
-            const int pb = (A + j) & 3;
-            mbar_wait(&p_empty[pb], (((A + j) >> 2) & 1) ^ 1);
-            load_base(A + j, s_p + pb * kAtomBytes, &p_full[pb]);
-          }
-          for (int j = 0; j < n; ++j) load_v(A + j);
+        for (int A = 0; A < n_atoms; ++A) {
+          load_base(A);
+          load_v(A);
         }
       }
     }
-  } else if (warp == 9) {
-    // =========================================== MMA issuer ===========================================
-    // The whole warp runs the control flow convergently (addresses / descriptors stay in the uniform datapath); only the
-    // tcgen05.mma / tcgen05.commit instructions themselves are issued by the elected lane.
-    const bool leader = elect_one();
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      auto advance = [&]() { if (++stage == p.ring_stages) { stage = 0; phase ^= 1; } };
-      // The issuing thread is on the critical path of every 64-key atom (each UMMA here is only 24-32 tensor cycles), so its
-      // instruction stream is kept minimal: descriptor high words are constants, low words advance by adds, loops are unrolled.
-      const uint32_t idesc_o = umma_idesc_f16(128, p.d_pad);
-      const uint32_t idesc_s = umma_idesc_f16(128, 64);
-      const uint64_t desc_hi = umma_desc_k_sw128(0);                       // everything except the 14-bit start address
-      const uint32_t ring_lo0 = (smem_u32(s_ring) & 0x3FFFF) >> 4;
-      const uint32_t stage_lo = static_cast<uint32_t>(p.ring_stage_bytes) >> 4;
-      const uint32_t q_lo = (smem_u32(s_q) & 0x3FFFF) >> 4;
-      const uint32_t p_lo0 = (smem_u32(s_p) & 0x3FFFF) >> 4;
-      uint32_t ring_lo = ring_lo0;                                         // descriptor low word of the current ring stage
-      auto advance2 = [&]() {
-        ring_lo += stage_lo;
-        if (++stage == p.ring_stages) { stage = 0; phase ^= 1; ring_lo = ring_lo0; }
-      };
-      const int ks_last = min(4, (p.d - (p.nd - 1) * 64 + 15) / 16);     // k-steps of the last 64-wide head-dim chunk
-      // Consecutive tcgen05.mma into the SAME accumulator serialise on the tensor pipe's accumulate latency (measured ~180 cycles per
-      // dependent M128xN64 / N48 instruction), so atoms are issued in PAIRS with their k-steps interleaved: S(A), S(A+1) target two S
-      // buffers and PV(A), PV(A+1) two O accumulators (O0 even atoms, O1 odd atoms, summed in the epilogue) -> 2 independent chains.
-      const bool dual = p.d_pad <= 128 && n_atoms >= 2;
-      const uint32_t tmem_o1 = dual ? tmem_o + 128 : tmem_o;
-      int g = 0;  // S-tile counter across both passes
-      auto issue_s_pair = [&](int A0) {
-        const int n = min(2, n_atoms - A0);
-        const int sb0 = g & 3, sb1 = (g + 1) & 3;
-        FZ_TIMED(0, mbar_wait(&s_empty[sb0], ((g >> 2) & 1) ^ 1));
-        if (n == 2) FZ_TIMED(0, mbar_wait(&s_empty[sb1], (((g + 1) >> 2) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + sb0 * 64, d1 = tmem_base + sb1 * 64;
-        uint32_t a_lo = q_lo;
-        for (int c = 0; c < p.nd; ++c) {
-          FZ_TIMED(1, mbar_wait(&ring_full[stage], phase));
-          const uint32_t lo0 = ring_lo;
-          uint64_t* e0 = &ring_empty[stage];
-          advance2();
-          uint32_t lo1 = lo0;
-          uint64_t* e1 = e0;
-          if (n == 2) {
-            FZ_TIMED(1, mbar_wait(&ring_full[stage], phase));
-            lo1 = ring_lo;
-            e1 = &ring_empty[stage];
-            advance2();
-          }
-          tc_fence_after();
-          const int ksteps = (c == p.nd - 1) ? ks_last : 4;
-          const long long _tm0 = dbg_on ? clock64() : 0;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (leader && k < ksteps) {
-              umma_f16_ss(d0, desc_hi | (a_lo + 2 * k), desc_hi | (lo0 + 2 * k), idesc_s, (c | k) ? 1u : 0u);
-              if (n == 2) umma_f16_ss(d1, desc_hi | (a_lo + 2 * k), desc_hi | (lo1 + 2 * k), idesc_s, (c | k) ? 1u : 0u);
-            }
-          }
-          const long long _tm1 = dbg_on ? clock64() : 0;
-          if (leader) {
-            umma_commit(e0);
-            if (n == 2) umma_commit(e1);
-          }
-          if (dbg_on) { dbg_acc[5] += _tm1 - _tm0; dbg_acc[6] += clock64() - _tm1; }
-          a_lo += kAtomBytes >> 4;
-        }
-        if (leader) {
-          umma_commit(&s_full[sb0]);
-          if (n == 2) umma_commit(&s_full[sb1]);
-        }
-        __syncwarp();
-        g += n;
-      };
-      auto issue_pv_pair = [&](int A0) {
-        const int n = min(2, n_atoms - A0);
-        const int pb0 = A0 & 3, pb1 = (A0 + 1) & 3;
-        FZ_TIMED(2, mbar_wait(&p_full[pb0], (A0 >> 2) & 1));
-        if (n == 2) FZ_TIMED(2, mbar_wait(&p_full[pb1], ((A0 + 1) >> 2) & 1));
-        FZ_TIMED(3, mbar_wait(&ring_full[stage], phase));
-        const uint32_t v0 = ring_lo;
-        uint64_t* e0 = &ring_empty[stage];
-        advance2();
-        uint32_t v1 = v0;
-        uint64_t* e1 = e0;
-        if (n == 2) {
-          FZ_TIMED(3, mbar_wait(&ring_full[stage], phase));
-          v1 = ring_lo;
-          e1 = &ring_empty[stage];
-          advance2();
-        }
-        tc_fence_after();
-        const uint32_t a0 = p_lo0 + pb0 * (kAtomBytes >> 4), a1 = p_lo0 + pb1 * (kAtomBytes >> 4);
-        const long long _tp0 = dbg_on ? clock64() : 0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          if (leader) {
-            umma_f16_ss(tmem_o, desc_hi | (a0 + 2 * k), desc_hi | (v0 + 2 * k), idesc_o, (A0 | k) ? 1u : 0u);
-            if (n == 2) umma_f16_ss(tmem_o1, desc_hi | (a1 + 2 * k), desc_hi | (v1 + 2 * k), idesc_o, (dual ? (A0 | k) : 1) ? 1u : 0u);
-          }
-        }
-        if (dbg_on) dbg_acc[7] += clock64() - _tp0;
-        if (leader) {
-          umma_commit(e0);
-          umma_commit(&p_empty[pb0]);
-          if (n == 2) {
-            umma_commit(e1);
-            umma_commit(&p_empty[pb1]);
-          }
-        }
-        __syncwarp();
-      };
-      if (!replace) {
-        mbar_wait(q_full, 0);
-        tc_fence_after();
-        for (int A = 0; A < n_atoms; A += 2) issue_s_pair(A);
-        issue_s_pair(0);
-        for (int A = 0; A < n_atoms; A += 2) {
-          if (A + 2 < n_atoms) issue_s_pair(A + 2);
-          issue_pv_pair(A);
-        }
-      } else {
-        for (int A = 0; A < n_atoms; A += 2) issue_pv_pair(A);
-      }
-      if (leader) umma_commit(o_full);
-      if (dbg_on && leader) {
-        for (int i = 0; i < 4; ++i) p.dbg[i] = dbg_acc[i];
-        p.dbg[4] = clock64() - dbg_t0;
-        p.dbg[25] = dbg_acc[5]; p.dbg[26] = dbg_acc[6]; p.dbg[27] = dbg_acc[7];
+    return;
+  }
 
+  // =========================================== consumer warpgroups ===========================================
+  const int wg = warp >> 2;
+  const int st = threadIdx.x & 127;
+  const int warp_in = warp & 3;
+  // fragment of this thread: rows rl[h] = 16 warp_in + lane / 4 + 8 h of the warpgroup's 64, key / output column 8 i + c_base + j
+  // at register 4 i + 2 h + j (fz_wgmma.cuh)
+  const int c_base = 2 * (lane & 3);
+  int rl[2], q[2];
+  bool row_ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    rl[h] = 16 * warp_in + (lane >> 2) + 8 * h;
+    q[h] = q0 + 64 * wg + rl[h];
+    row_ok[h] = q[h] < p.S_q;
+  }
+  const uint64_t desc0 = wgmma_desc_k_sw128(smem_u32(smem));
+  auto desc_of = [&](const uint8_t* ptr) { return desc0 + static_cast<uint32_t>((ptr - smem) >> 4); };
+  int stage = 0;
+  uint32_t phase = 0;
+  auto release = [&]() {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&ring_empty[stage]);
+    if (++stage == p.ring_stages) { stage = 0; phase ^= 1; }
+  };
+  const float sc2 = p.scale_log2;
+  // S[64 x 64 keys] = Q K^T of atom A (head-dim columns beyond d are TMA zero fill), keys outside the valid range set to -inf
+  auto scores = [&](float (&s)[32], int A) {
+    for (int c = 0; c < p.nd; ++c) {
+      mbar_wait(&ring_full[stage], phase);
+      const uint64_t da = desc_of(s_q + c * kAtomBytes + wg * kHalfAtom);
+      const uint64_t db = desc_of(s_ring + stage * p.ring_stage_bytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_f16<64>(s, da + 2 * k, db + 2 * k, (c | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      release();
+    }
+    if (p.masked) {
+      const AtomInfo ai = atom_info(p, atoms_per_slot, A);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const int e = 8 * i + c_base + j;
+            if (e >= ai.valid || (p.causal && ai.k0 + e > q[h])) s[4 * i + 2 * h + j] = -INFINITY;
+          }
+    }
+  };
+
+  float o[32 * NCH];
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  if (!replace) {
+    mbar_wait(q_full, 0);
+    // ------------------------------ pass 1 (hooked rows): row max and sum of exponentials ------------------------------
+    for (int A = 0; exact && A < n_atoms; ++A) {
+      float s[32];
+      scores(s, A);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float cm = -INFINITY;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) cm = fmaxf(cm, fmaxf(s[4 * i + 2 * h], s[4 * i + 2 * h + 1]));
+        cm = quad_max(cm);
+        const float m_new = fmaxf(m_run[h], cm);
+        if (m_new > -INFINITY) {
+          const float mb = m_new * sc2;
+          float a = 0.f;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) a += ex2(fmaf(s[4 * i + 2 * h], sc2, -mb)) + ex2(fmaf(s[4 * i + 2 * h + 1], sc2, -mb));
+          l_run[h] = l_run[h] * ex2((m_run[h] - m_new) * sc2) + a;  // per-thread partial: the quad shares m_run
+        }
+        m_run[h] = m_new;
       }
     }
-  } else {
-    // =========================================== softmax / epilogue warpgroups ===========================================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;  // query row within the tile == TMEM lane
-    const int q = q0 + row;
-    const bool row_ok = q < p.S_q;
-    const uint32_t lane_addr = static_cast<uint32_t>(quad * 32) << 16;
-    const int wg = warp >> 2;                  // handles atoms with (A & 1) == wg
-    const int st = threadIdx.x & 127;          // 0..127 within the warpgroup
-    float m_run = -INFINITY, l_run = 0.f;
-    if (!replace) {
-      // ------------------------------ pass 1: row max of the raw scores (and sum of exponentials when exact) ------------------------------
-      const float sc2 = p.scale_log2;
-      for (int A = wg; A < n_atoms; A += 2) {
-        const int g = A, sb = g & 3;
-        FZ_TIMED(0, mbar_wait(&s_full[sb], (g >> 2) & 1));
-        tc_fence_after();
-        const int valid = atom_info(p, atoms_per_slot, A).valid;
-        uint32_t r[64];
-        tmem_ld_32x32b_x32(tmem_base + lane_addr + sb * 64, reinterpret_cast<uint32_t(&)[32]>(r[0]));
-        tmem_ld_32x32b_x32(tmem_base + lane_addr + sb * 64 + 32, reinterpret_cast<uint32_t(&)[32]>(r[32]));
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_empty[sb]);  // scores are in registers: the MMA warp may overwrite this S tile
-        if constexpr (kMasked) {
-          if (valid < 64) {
+    float inv_l[2], mb2[2], mrow[2];
+    const float* xe = p.xedit;
+    const bool row_ops = row_mode == FZ_ATTN_CROSSEDIT || (p.acc && edited);
 #pragma unroll
-            for (int e = 0; e < 64; ++e)
-              if (e >= valid) r[e] = 0xff800000u;  // -inf
-          }
-          if (p.causal) {
-            const int k0c = atom_info(p, atoms_per_slot, A).k0;
+    for (int h = 0; h < 2; ++h) {
+      inv_l[h] = exact ? 1.0f / quad_sum(l_run[h]) : 1.0f;
+      mb2[h] = exact ? m_run[h] * sc2 : 0.f;
+      mrow[h] = blend ? p.mask[static_cast<long long>(fc) * p.S_q + min(q[h], p.S_q - 1)] : 1.f;
+      l_run[h] = 0.f;
+    }
+    // ------------------------ pass 2 (the only pass of un-hooked rows): probabilities -> P tile (-> cache) -> O += P V ------------------------
+    for (int A = 0; A < n_atoms; ++A) {
+      const AtomInfo ai = atom_info(p, atoms_per_slot, A);
+      float pv[32];
+      scores(pv, A);
+      if (!exact) {
 #pragma unroll
-            for (int e = 0; e < 64; ++e)
-              if (k0c + e > q) r[e] = 0xff800000u;
-          }
-        }
-        float c0 = -INFINITY, c1 = -INFINITY, c2 = -INFINITY, c3 = -INFINITY;
+        for (int h = 0; h < 2; ++h) {
+          float cm = -INFINITY;
 #pragma unroll
-        for (int e = 0; e < 64; e += 4) {
-          c0 = fmaxf(c0, __uint_as_float(r[e + 0]));
-          c1 = fmaxf(c1, __uint_as_float(r[e + 1]));
-          c2 = fmaxf(c2, __uint_as_float(r[e + 2]));
-          c3 = fmaxf(c3, __uint_as_float(r[e + 3]));
-        }
-        const float cm = fmaxf(fmaxf(c0, c1), fmaxf(c2, c3));
-        if (exact) {
-          const float m_new = fmaxf(m_run, cm);
-          if (m_new > -INFINITY) {
-            const float mb = m_new * sc2;
-            float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+          for (int i = 0; i < 8; ++i) cm = fmaxf(cm, fmaxf(pv[4 * i + 2 * h], pv[4 * i + 2 * h + 1]));
+          cm = quad_max(cm);
+          if (m_run[h] == -INFINITY ? cm > -INFINITY : (cm - m_run[h]) * sc2 > kRescaleThreshold) {
+            // the PV of the previous atom has completed (wgmma_wait below): O and l of this row are rescaled to the new reference
+            const float f = ex2((m_run[h] - cm) * sc2);
+            l_run[h] *= f;
+            if (A > 0) {
 #pragma unroll
-            for (int e = 0; e < 64; e += 4) {
-              a0 += ex2(fmaf(__uint_as_float(r[e + 0]), sc2, -mb));
-              a1 += ex2(fmaf(__uint_as_float(r[e + 1]), sc2, -mb));
-              a2 += ex2(fmaf(__uint_as_float(r[e + 2]), sc2, -mb));
-              a3 += ex2(fmaf(__uint_as_float(r[e + 3]), sc2, -mb));
+              for (int i = 0; i < 8 * NCH; ++i) { o[4 * i + 2 * h] *= f; o[4 * i + 2 * h + 1] *= f; }
             }
-            l_run = l_run * ex2((m_run - m_new) * sc2) + ((a0 + a1) + (a2 + a3));
+            m_run[h] = cm;
+            mb2[h] = cm * sc2;
           }
-          m_run = m_new;
-        } else {
-          m_run = fmaxf(m_run, cm);
         }
       }
-      // merge the two warpgroups' running (max, sum); also orders every pass-1 barrier phase before pass 2
-      xchg[(wg * 128 + row) * 2 + 0] = m_run;
-      xchg[(wg * 128 + row) * 2 + 1] = l_run;
-      named_bar_sync(3, 256);
-      {
-        const float m_o = xchg[((wg ^ 1) * 128 + row) * 2 + 0], l_o = xchg[((wg ^ 1) * 128 + row) * 2 + 1];
-        const float m_new = fmaxf(m_run, m_o);
-        if (exact) l_run = l_run * ex2((m_run - m_new) * sc2) + l_o * ex2((m_o - m_new) * sc2);
-        m_run = m_new;
-      }
-      named_bar_sync(3, 256);
-      const long long dbg_p1 = clock64() - dbg_t0;
-      const float inv_l = exact ? (1.0f / l_run) : 1.0f;
-      const float mb2 = m_run * sc2;
-      float lf0 = 0.f, lf1 = 0.f, lf2 = 0.f, lf3 = 0.f;
-      const float mrow = blend ? p.mask[static_cast<long long>(fc) * p.S_q + min(q, p.S_q - 1)] : 1.f;
-      const float* xe = p.xedit;
-      const bool row_ops = row_mode == FZ_ATTN_CROSSEDIT || (p.acc && edited);
-      // ------------------------------ pass 2: probabilities -> P tile (-> cache) ------------------------------
-      for (int A = wg; A < n_atoms; A += 2) {
-        const int g = n_atoms + A, sb = g & 3, pb = A & 3;
-        const AtomInfo ai = atom_info(p, atoms_per_slot, A);
-        FZ_TIMED(1, mbar_wait(&s_full[sb], (g >> 2) & 1));
-        tc_fence_after();
-        uint32_t r[64];
-        tmem_ld_32x32b_x32(tmem_base + lane_addr + sb * 64, reinterpret_cast<uint32_t(&)[32]>(r[0]));
-        tmem_ld_32x32b_x32(tmem_base + lane_addr + sb * 64 + 32, reinterpret_cast<uint32_t(&)[32]>(r[32]));
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_empty[sb]);
-        if constexpr (kMasked) {
-          if (ai.valid < 64) {
 #pragma unroll
-            for (int e = 0; e < 64; ++e)
-              if (e >= ai.valid) r[e] = 0xff800000u;
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            float& x = pv[4 * i + 2 * h + j];
+            x = ex2(fmaf(x, sc2, -mb2[h]));
+            if (exact) x *= inv_l[h];
+            else l_run[h] += x;
           }
-          if (p.causal) {
+      if (row_ops) {
 #pragma unroll
-            for (int e = 0; e < 64; ++e)
-              if (ai.k0 + e > q) r[e] = 0xff800000u;
-          }
-        }
-        float* pv = reinterpret_cast<float*>(r);
-        if (exact) {
+        for (int h = 0; h < 2; ++h) {
+          // key index n = ai.k0 + 8 i + c_base + j (single slot).  cur = fp16(p); optional running sum; optional edit (in fp32, one rounding)
+          const long long rbase = ((static_cast<long long>(fc) * p.heads + head) * p.S_q + min(q[h], p.S_q - 1));
+          if (p.acc && row_ok[h]) {
+            __half* ap = p.acc + rbase * p.acc_ld;
 #pragma unroll
-          for (int e = 0; e < 64; ++e) pv[e] = ex2(fmaf(pv[e], sc2, -mb2)) * inv_l;
-        } else {
-#pragma unroll
-          for (int e = 0; e < 64; ++e) pv[e] = ex2(fmaf(pv[e], sc2, -mb2));
-#pragma unroll
-          for (int e = 0; e < 64; e += 4) { lf0 += pv[e]; lf1 += pv[e + 1]; lf2 += pv[e + 2]; lf3 += pv[e + 3]; }
-        }
-        if (row_ops) {
-#pragma unroll
-          for (int c = 0; c < 64; c += 32) {
-            float* pc = pv + c;
-            // key index n = ai.k0 + c + e (single slot).  cur = fp16(p); optional running sum; optional edit (in fp32, one rounding)
-            const int n0 = ai.k0 + c;
-            const long long rbase = ((static_cast<long long>(fc) * p.heads + head) * p.S_q + min(q, p.S_q - 1));
-            if (p.acc && row_ok) {
-              __half* ap = p.acc + rbase * p.acc_ld + n0;
-#pragma unroll
-              for (int e = 0; e < 32; e += 8) {
-                if (n0 + e < p.acc_ld) {
-                  uint4 v = *reinterpret_cast<uint4*>(ap + e);
-                  __half* hv = reinterpret_cast<__half*>(&v);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) hv[j] = __float2half_rn(__half2float(hv[j]) + __half2float(__float2half_rn(pc[e + j])));
-                  *reinterpret_cast<uint4*>(ap + e) = v;
-                }
+            for (int i = 0; i < 8; ++i) {
+              const int n = ai.k0 + 8 * i + c_base;
+              if (n < p.acc_ld) {
+                const float2 a = __half22float2(*reinterpret_cast<__half2*>(ap + n));
+                const float c0 = __half2float(__float2half_rn(pv[4 * i + 2 * h])), c1 = __half2float(__float2half_rn(pv[4 * i + 2 * h + 1]));
+                *reinterpret_cast<__half2*>(ap + n) = __floats2half2_rn(a.x + c0, a.y + c1);
               }
             }
-            if (row_mode == FZ_ATTN_CROSSEDIT) {
-              const __half* brow = p.base_rows + rbase * p.base_ld;
-              const int xmode = static_cast<int>(xe[0]);  // 0 refine, 1 replace
-              const float* x_alpha = xe + 8;              // [80] cross_replace_alpha of this step
-              const float* x_eq = xe + 8 + 80;            // [80] equalizer (1 when absent)
-              const float* x_a = xe + 8 + 160;            // [80] refine alphas
-              const float* x_map = xe + 8 + 240;          // [80] refine mapper (as float)
-              const float* x_M = xe + 8 + 320;            // [80][80] replace matrix M[w][n]
-              float rr[32];
-              if (xmode == 1) {
+          }
+          if (row_mode == FZ_ATTN_CROSSEDIT) {
+            const __half* brow = p.base_rows + rbase * p.base_ld;
+            const int xmode = static_cast<int>(xe[0]);  // 0 refine, 1 replace
+            const float* x_alpha = xe + 8;              // [80] cross_replace_alpha of this step
+            const float* x_eq = xe + 8 + 80;            // [80] equalizer (1 when absent)
+            const float* x_a = xe + 8 + 160;            // [80] refine alphas
+            const float* x_map = xe + 8 + 240;          // [80] refine mapper (as float)
+            const float* x_M = xe + 8 + 320;            // [80][80] replace matrix M[w][n]
+            float rr[16];
+            if (xmode == 1) {
 #pragma unroll
-                for (int e = 0; e < 32; ++e) rr[e] = 0.f;
-                for (int w = 0; w < p.keys_per_slot; ++w) {
-                  const float bw = __half2float(brow[w]);
-                  const float* mrow_p = x_M + w * 80 + n0;
+              for (int e = 0; e < 16; ++e) rr[e] = 0.f;
+              for (int w = 0; w < p.keys_per_slot; ++w) {
+                const float bw = __half2float(brow[w]);
+                const float* mrow_p = x_M + w * 80;
 #pragma unroll
-                  for (int e = 0; e < 32; ++e)
-                    if (n0 + e < 80) rr[e] += bw * __ldg(mrow_p + e);
-                }
+                for (int i = 0; i < 8; ++i)
+#pragma unroll
+                  for (int j = 0; j < 2; ++j) {
+                    const int n = ai.k0 + 8 * i + c_base + j;
+                    if (n < 80) rr[2 * i + j] += bw * __ldg(mrow_p + n);
+                  }
               }
+            }
 #pragma unroll
-              for (int e = 0; e < 32; ++e) {
-                const int n = n0 + e;
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+              for (int j = 0; j < 2; ++j) {
+                const int n = ai.k0 + 8 * i + c_base + j;
                 if (n < p.keys_per_slot) {
-                  const float cur = __half2float(__float2half_rn(pc[e]));
+                  float& x = pv[4 * i + 2 * h + j];
+                  const float cur = __half2float(__float2half_rn(x));
                   float R;
-                  if (xmode == 1) R = rr[e];
+                  if (xmode == 1) R = rr[2 * i + j];
                   else {
                     int mi = static_cast<int>(__ldg(x_map + n));
                     if (mi < 0) mi += p.keys_per_slot;  // python negative index (masked by a[n] == 0)
@@ -573,665 +395,83 @@ __global__ void __launch_bounds__(320, 1) attn_kernel(const __grid_constant__ At
                   }
                   R *= __ldg(x_eq + n);
                   const float al = __ldg(x_alpha + n);
-                  pc[e] = R * al + (1.f - al) * cur;
+                  x = R * al + (1.f - al) * cur;
                 }
               }
+          }
+        }
+      }
+      // P buffer pb of this warpgroup: its PV two atoms ago is complete (wgmma_wait below); for STORE its TMA store must be done reading
+      const int pb = A & 1;
+      uint8_t* ptile = s_p + (wg * 2 + pb) * kHalfAtom;
+      if (row_mode == FZ_ATTN_STORE) {
+        if (st == 0) tma_store_wait_read<1>();
+        named_bar_sync(1 + wg, 128);
+      }
+      // swizzled stores: 16-byte chunk i of row r lands at chunk (i ^ (r & 7))
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          *reinterpret_cast<uint32_t*>(ptile + rl[h] * 128 + ((i ^ (rl[h] & 7)) << 4) + c_base * 2) =
+              pack_half2(pv[4 * i + 2 * h], pv[4 * i + 2 * h + 1]);
+      if (blend) {
+        mbar_wait(&base_full[A & 1], (A >> 1) & 1);
+        const uint8_t* btile = s_base + (A & 1) * kAtomBytes + wg * kHalfAtom;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (mrow[h] == 0.f) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int off = rl[h] * 128 + ((i ^ (rl[h] & 7)) << 4) + c_base * 2;
+              *reinterpret_cast<uint32_t*>(ptile + off) = *reinterpret_cast<const uint32_t*>(btile + off);
             }
           }
         }
-        // the P buffer must be free: its previous PV MMA done (p_empty) and, for STORE, its previous TMA store done reading
-        if (row_mode == FZ_ATTN_STORE && st == 0) tma_store_wait_read<1>();
-        FZ_TIMED(2, mbar_wait(&p_empty[pb], ((A >> 2) & 1) ^ 1));
-        FZ_TIMED(3, named_bar_sync(1 + wg, 128));
-        uint8_t* prow = s_p + pb * kAtomBytes + row * 128;
-        // swizzled 16-byte stores: chunk j of row `row` lands at chunk (j ^ (row & 7))
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&base_empty[A & 1]);
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1 + wg, 128);
+      if (row_mode == FZ_ATTN_STORE && st == 0) {
+        tma_store_5d(&p.tmStore, ptile, ai.k0, ai.slot, q0 + 64 * wg, head, fc);
+        tma_store_commit();
+      }
+      mbar_wait(&ring_full[stage], phase);
+      wgmma_fence();
+      pv_mma<NCH>(o, desc_of(ptile), desc_of(s_ring + stage * p.ring_stage_bytes), A ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      release();
+    }
 #pragma unroll
-        for (int e = 0; e < 64; e += 8) {
-          uint4 v;
-          v.x = pack_half2(pv[e + 0], pv[e + 1]);
-          v.y = pack_half2(pv[e + 2], pv[e + 3]);
-          v.z = pack_half2(pv[e + 4], pv[e + 5]);
-          v.w = pack_half2(pv[e + 6], pv[e + 7]);
-          const int j = e >> 3;
-          *reinterpret_cast<uint4*>(prow + ((j ^ (row & 7)) << 4)) = v;
-        }
-        if (blend) {
-          mbar_wait(&base_full[wg], (A >> 1) & 1);
-          if (mrow == 0.f) {
-            const uint8_t* srow = s_pbase + wg * kAtomBytes + row * 128;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) *reinterpret_cast<uint4*>(prow + j * 16) = *reinterpret_cast<const uint4*>(srow + j * 16);
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&base_empty[wg]);
-        }
-        fence_proxy_async_smem();
-        FZ_TIMED(4, named_bar_sync(1 + wg, 128));
-        if (st == 0) {
-          if (row_mode == FZ_ATTN_STORE) {
-            tma_store_5d(&p.tmStore, s_p + pb * kAtomBytes, ai.k0, ai.slot, q0, head, fc);
-            tma_store_commit();
-          }
-          mbar_arrive(&p_full[pb]);
-        }
-      }
-      if (dbg_on && warp == 0 && lane == 0) p.dbg[24] = dbg_p1;
-      if (!exact) {
-        l_run = (lf0 + lf1) + (lf2 + lf3);
-        xchg[(wg * 128 + row) * 2] = l_run;
-        named_bar_sync(3, 256);
-        l_run += xchg[((wg ^ 1) * 128 + row) * 2];
-      }
-    }
-    // ------------------------------ epilogue: O (TMEM) -> fp16 -> global (16-column chunks alternate between the warpgroups) ------------------------------
-    if (dbg_on && (warp == 0 || warp == 4)) dbg_acc[6] = clock64() - dbg_t0;  // end of pass 2
-    FZ_TIMED(5, mbar_wait(o_full, 0));
-    tc_fence_after();
-    const float o_scale = (!replace && !exact) ? (1.0f / l_run) : 1.0f;
-    __half* orow = p.out + (static_cast<long long>(bf) * p.S_q + min(q, p.S_q - 1)) * p.ldo + head * p.d;
-    const bool dual_o = p.d_pad <= 128 && n_atoms >= 2;  // odd atoms accumulated into a second O tile at +128 columns
-#pragma unroll 1
-    for (int c = wg * 16; c < p.d_pad; c += 32) {
-      uint32_t r[16];
-      tmem_ld_32x32b_x16(tmem_o + lane_addr + c, r);
-      if (dual_o) {
-        uint32_t r1[16];
-        tmem_ld_32x32b_x16(tmem_o + 128 + lane_addr + c, r1);
-        tmem_ld_wait();
-#pragma unroll
-        for (int e = 0; e < 16; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) + __uint_as_float(r1[e]));
-      }
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int e = 0; e < 16; e += 8) {
-          if (c + e < p.d) {
-            uint4 v;
-            v.x = pack_half2(__uint_as_float(r[e + 0]) * o_scale, __uint_as_float(r[e + 1]) * o_scale);
-            v.y = pack_half2(__uint_as_float(r[e + 2]) * o_scale, __uint_as_float(r[e + 3]) * o_scale);
-            v.z = pack_half2(__uint_as_float(r[e + 4]) * o_scale, __uint_as_float(r[e + 5]) * o_scale);
-            v.w = pack_half2(__uint_as_float(r[e + 6]) * o_scale, __uint_as_float(r[e + 7]) * o_scale);
-            *reinterpret_cast<uint4*>(orow + c + e) = v;
-          }
-        }
-      }
-    }
-    if (row_mode == FZ_ATTN_STORE && st == 0) tma_store_wait_all<0>();
-    if (dbg_on && lane == 0 && (warp == 0 || warp == 4)) {
-      const int base = warp == 0 ? 8 : 16;
-      for (int i = 0; i < 7; ++i) p.dbg[base + i] = dbg_acc[i];
-      p.dbg[base + 7] = clock64() - dbg_t0;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Plain attention (no controller hook on any row) for head dims <= 64: the 64x64-latent spatio-temporal self-attention layers
-// (attention_register.py:131-218 with q.shape[1] > 32**2, which the controller leaves untouched: attention_store.py:58-59), i.e.
-// 3/4 of the attention time of a DDIM step.  Nothing has to be stored or edited here, so the probabilities need not be
-// normalised before PV: ONE pass over the keys with a running row maximum (online softmax),
-//   p = exp2(s*c - m_ref*c) rounded to fp16 for PV (fp32 row sum l), O / l at the end,
-// where m_ref is the row's reference maximum.  It is only raised (and O, l rescaled by 2^((m_old - m_new) c)) when a tile's maximum
-// exceeds it by more than 8 in the log2 domain, so the rescale is rare and p <= 2^8 stays far inside fp16 range; the result is the
-// same softmax(QK^T)V, the fp16 rounding of p merely happens at a power-of-two different scale.
-// Pipeline (built for the small head dim, where the MMA issue rate and shared-memory operand reads bound the tensor pipe):
-//   * key tiles of 128: QK^T as M128 x N128 UMMAs (with N=64 the A operand re-read from shared memory bounds the MMA: measured
-//     48 clk per N=64 K=16 instruction instead of 32, tools/micro/umma_rate.cu)
-//   * P never touches shared memory: the softmax warps overwrite the S columns in TMEM with packed fp16 (tcgen05.st) and the PV
-//     UMMA takes its A operand from TMEM (measured 24 clk per N=48 instruction instead of 44 from shared memory)
-//   * three S/P buffers rotate over two softmax warpgroups (tile j -> buffer j % 3, warpgroup j & 1).  Each warpgroup owns its own
-//     (m_ref, l, O accumulator): a rescale touches only the warpgroup's own O between two of its own PV MMAs, and the two partial
-//     results are merged in the epilogue (split-KV).  tcgen05.mma executes in issue order, so QK(j+3) is issued right behind PV(j)
-//     into the buffer it frees: no "S empty" barrier.
-// TMEM: S/P buffers at columns 0 / 128 / 256, O of warpgroup 0 at 384, of warpgroup 1 at 448.
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int kPlainStageBytes = 16384;
-constexpr int kPlainStages = 10;
-constexpr int kPlainSmem = 1024 + kAtomBytes + kPlainStages * kPlainStageBytes + 4096;
-constexpr float kRescaleThreshold = 8.0f;  // log2 units
-#ifndef FZ_POLY_SEL
-#define FZ_POLY_SEL(e) (((e) & 3) == 3)  // which exponentials of a 32-chunk take the FMA-pipe polynomial (measured optimum: 1 in 4)
-#endif
-
-// kMasked: the last key tile of a slot may be partial (77 text keys at head dims the streaming cross kernel does not take); the full-tile
-// instantiation carries no masking code at all — with it in the loop the r = 64 self-attention ran 965 us instead of 820 us (ncu).
-template <bool kMasked>
-__global__ void __launch_bounds__(320, 1) attn_plain_kernel(const __grid_constant__ AttnParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  pdl_launch_dependents();
-  const int q0 = blockIdx.x * 128;
-  const int head = blockIdx.y;
-  const int bf = blockIdx.z;
-
-  uint8_t* s_q = smem;
-  uint8_t* s_ring = s_q + kAtomBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_ring + kPlainStages * kPlainStageBytes);
-  uint64_t* ring_full = bars;                     // [kPlainStages]
-  uint64_t* ring_empty = bars + kPlainStages;     // [kPlainStages]
-  uint64_t* q_full = bars + 2 * kPlainStages;
-  uint64_t* s_full = q_full + 1;                  // [3]
-  uint64_t* p_full = s_full + 3;                  // [3]
-  uint64_t* pv_done = p_full + 3;                 // [2] one per warpgroup: its latest PV has been accumulated
-  uint64_t* o_full = pv_done + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
-  float* xchg = reinterpret_cast<float*>(o_full + 2);  // [2 warpgroups][128 rows][2]
-
-  const int tiles_per_slot = (p.keys_per_slot + 127) >> 7;  // a partial last tile (text cross-attention: 77 keys) is masked below
-  const int n_tiles = tiles_per_slot * p.n_slots;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&p.tmQ);
-    tma_prefetch_desc(&p.tmK2);
-    tma_prefetch_desc(&p.tmVt);
-    for (int s = 0; s < kPlainStages; ++s) {
-      mbar_init(&ring_full[s], 1);
-      mbar_init(&ring_empty[s], 1);
-    }
-    mbar_init(q_full, 1);
-    for (int b = 0; b < 3; ++b) {
-      mbar_init(&s_full[b], 1);
-      mbar_init(&p_full[b], 4);
-    }
-    mbar_init(&pv_done[0], 1);
-    mbar_init(&pv_done[1], 1);
-    mbar_init(o_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == 9) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();  // prologue above overlaps the previous kernel's tail (programmatic dependent launch)
-  const uint32_t tmem_o = tmem_base + 384;  // + 64 * warpgroup
-  const int vt_atom_bytes = p.d_pad * 128;
-#ifdef FZ_ATTN_PROFILE
-  const bool dbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;  // warp-uniform
-#else
-  constexpr bool dbg_on = false;
-#endif
-  long long dbg_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  const long long dbg_t0 = clock64();
-
-  if (warp == 8) {
-    // =========================================== TMA producer ===========================================
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      auto advance = [&]() { if (++stage == kPlainStages) { stage = 0; phase ^= 1; } };
-      auto load_k = [&](int j) {
-        const int slot = j / tiles_per_slot, k0 = (j - slot * tiles_per_slot) << 7;
-        mbar_wait(&ring_empty[stage], phase ^ 1);
-        mbar_expect_tx(&ring_full[stage], 128 * 128);
-        tma_load_4d(s_ring + stage * kPlainStageBytes, &p.tmK2, &ring_full[stage], 0, head, k0, p.src_index[slot][bf]);
-        advance();
-      };
-      auto load_v = [&](int j) {
-        const int slot = j / tiles_per_slot, k0 = (j - slot * tiles_per_slot) << 7;
-        mbar_wait(&ring_empty[stage], phase ^ 1);
-        mbar_expect_tx(&ring_full[stage], 2 * vt_atom_bytes);
-        uint8_t* dst = s_ring + stage * kPlainStageBytes;
-        tma_load_4d(dst, &p.tmVt, &ring_full[stage], k0, 0, head, p.src_index[slot][bf]);
-        tma_load_4d(dst + vt_atom_bytes, &p.tmVt, &ring_full[stage], k0 + 64, 0, head, p.src_index[slot][bf]);
-        advance();
-      };
-      mbar_expect_tx(q_full, kAtomBytes);
-      tma_load_4d(s_q, &p.tmQ, q_full, 0, head, q0, bf);
-      for (int j = 0; j < min(3, n_tiles); ++j) load_k(j);  // same order as the MMA warp consumes
-      for (int j = 0; j < n_tiles; ++j) {
-        load_v(j);
-        if (j + 3 < n_tiles) load_k(j + 3);
-      }
-    }
-  } else if (warp == 9) {
-    // =========================================== MMA issuer ===========================================
-    const bool leader = elect_one();
-    int stage = 0;
-    uint32_t phase = 0;
-    const uint32_t idesc_s = umma_idesc_f16(128, 128);
-    const uint32_t idesc_o = umma_idesc_f16(128, p.d_pad);
-    const uint64_t desc_hi = umma_desc_k_sw128(0);
-    const uint32_t ring_lo0 = (smem_u32(s_ring) & 0x3FFFF) >> 4;
-    const uint32_t q_lo = (smem_u32(s_q) & 0x3FFFF) >> 4;
-    const uint32_t vt_atom_lo = static_cast<uint32_t>(vt_atom_bytes) >> 4;
-    uint32_t ring_lo = ring_lo0;
-    auto advance = [&]() {
-      ring_lo += kPlainStageBytes >> 4;
-      if (++stage == kPlainStages) { stage = 0; phase ^= 1; ring_lo = ring_lo0; }
-    };
-    const int ksteps = (p.d + 15) >> 4;
-    auto issue_qk = [&](int b) {
-      FZ_TIMED(1, mbar_wait(&ring_full[stage], phase));
-      tc_fence_after();
-      if (leader) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          if (k < ksteps) umma_f16_ss(tmem_base + b * 128, desc_hi | (q_lo + 2 * k), desc_hi | (ring_lo + 2 * k), idesc_s, k ? 1u : 0u);
-        umma_commit(&ring_empty[stage]);
-        umma_commit(&s_full[b]);
-      }
-      __syncwarp();
-      advance();
-    };
-    mbar_wait(q_full, 0);
-    tc_fence_after();
-    for (int j = 0; j < min(3, n_tiles); ++j) issue_qk(j);
-    int b = 0;
-    for (int j = 0; j < n_tiles; ++j) {
-      const int wg = j & 1;
-      FZ_TIMED(2, mbar_wait(&p_full[b], (j / 3) & 1));
-      FZ_TIMED(3, mbar_wait(&ring_full[stage], phase));
-      tc_fence_after();
-      if (leader) {
-        const uint32_t a0 = tmem_base + b * 128;
-        const uint32_t od = tmem_o + wg * 64;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t bdesc = desc_hi | (ring_lo + (k >> 2) * vt_atom_lo + 2 * (k & 3));
-          umma_f16_ts(od, a0 + k * 8, bdesc, idesc_o, (j >= 2 || k) ? 1u : 0u);
-        }
-        umma_commit(&ring_empty[stage]);
-        umma_commit(&pv_done[wg]);
-      }
-      __syncwarp();
-      advance();
-      if (j + 3 < n_tiles) issue_qk(b);  // executes behind PV(j) on the tensor pipe: reuses the buffer PV(j) just read
-      b = (b == 2) ? 0 : b + 1;
-    }
-    if (leader) umma_commit(o_full);
-    __syncwarp();
-    if (dbg_on && leader) {
-      for (int i = 0; i < 4; ++i) p.dbg[i] = dbg_acc[i];
-      p.dbg[4] = clock64() - dbg_t0;
-    }
+    for (int h = 0; h < 2; ++h) l_run[h] = quad_sum(l_run[h]);
   } else {
-    // =========================================== softmax / epilogue warpgroups ===========================================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(quad * 32) << 16;
-    const int wg = warp >> 2;
-    const float sc2 = p.scale_log2;
-    const uint32_t my_o = tmem_o + wg * 64 + lane_addr;
-    float m_ref = -INFINITY;
-    float lf0 = 0.f, lf1 = 0.f, lf2 = 0.f, lf3 = 0.f;
-    int t = 0;  // tiles this warpgroup has finished
-    for (int j = wg; j < n_tiles; j += 2, ++t) {
-      const int b = j % 3;
-      FZ_TIMED(1, mbar_wait(&s_full[b], (j / 3) & 1));
-      tc_fence_after();
-      const uint32_t sbase = tmem_base + lane_addr + b * 128;
-      const int tile_valid = kMasked ? min(128, p.keys_per_slot - ((j % tiles_per_slot) << 7)) : 128;  // keys beyond it are TMA zero fill: masked to -inf
-      uint32_t ra[32], rb[32];
-      // ---- tile maximum (TMEM reads are cheap: the scores are read again below instead of being kept in 128 registers) ----
-      {
-        float c0 = -INFINITY, c1 = -INFINITY, c2 = -INFINITY, c3 = -INFINITY;
-        tmem_ld_32x32b_x32(sbase, ra);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint32_t(&cur)[32] = (i & 1) ? rb : ra;
-          uint32_t(&nxt)[32] = (i & 1) ? ra : rb;
-          if (i < 3) tmem_ld_32x32b_x32(sbase + (i + 1) * 32, nxt);
-          if constexpr (kMasked) {
-            if (tile_valid < (i + 1) * 32) {
-#pragma unroll
-              for (int e = 0; e < 32; ++e)
-                if (i * 32 + e >= tile_valid) cur[e] = 0xff800000u;
-            }
-          }
-#pragma unroll
-          for (int e = 0; e < 32; e += 8) {
-            c0 = fmaxf(fmaxf(c0, __uint_as_float(cur[e + 0])), __uint_as_float(cur[e + 1]));
-            c1 = fmaxf(fmaxf(c1, __uint_as_float(cur[e + 2])), __uint_as_float(cur[e + 3]));
-            c2 = fmaxf(fmaxf(c2, __uint_as_float(cur[e + 4])), __uint_as_float(cur[e + 5]));
-            c3 = fmaxf(fmaxf(c3, __uint_as_float(cur[e + 6])), __uint_as_float(cur[e + 7]));
-          }
-          if (i < 3) tmem_ld_wait();
-        }
-        const float tmax = fmaxf(fmaxf(c0, c1), fmaxf(c2, c3));
-        // first chunk of the exp pass goes in flight before the (rare) rescale
-        tmem_ld_32x32b_x32(sbase, ra);
-        if (t == 0) {
-          m_ref = tmax;
-        } else {
-          const bool need = (tmax - m_ref) * sc2 > kRescaleThreshold;
-          if (__any_sync(0xffffffffu, need)) {
-            // this warpgroup's previous PV must have been accumulated; nothing else touches its O until p_full below
-            FZ_TIMED(0, mbar_wait(&pv_done[wg], (t - 1) & 1));
-            tc_fence_after();
-            const float m_new = need ? tmax : m_ref;
-            const float f = ex2((m_ref - m_new) * sc2);
-            m_ref = m_new;
-            lf0 *= f; lf1 *= f; lf2 *= f; lf3 *= f;
-            for (int c = 0; c < p.d_pad; c += 16) {
-              uint32_t o[16];
-              tmem_ld_32x32b_x16(my_o + c, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int e = 0; e < 16; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * f);
-              tmem_st_32x32b_x16(my_o + c, o);
-            }
-          }
-        }
-        tmem_ld_wait();
-      }
-      const float mb2 = m_ref * sc2;
-      // ---- probabilities: 32-column chunks, software pipelined (load of chunk i+1 in flight during FFMA -> MUFU -> pack of chunk i);
-      //      keys [32i, 32i+32) -> packed columns [16i, 16i+16), which lie inside score columns that were already read ----
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint32_t(&cur)[32] = (i & 1) ? rb : ra;
-        uint32_t(&nxt)[32] = (i & 1) ? ra : rb;
-        if (i < 3) tmem_ld_32x32b_x32(sbase + (i + 1) * 32, nxt);
-        if constexpr (kMasked) {
-          if (tile_valid < (i + 1) * 32) {
-#pragma unroll
-            for (int e = 0; e < 32; ++e)
-              if (i * 32 + e >= tile_valid) cur[e] = 0xff800000u;  // exp2(-inf) = 0 on both the MUFU and the polynomial path
-          }
-        }
-        float* pv = reinterpret_cast<float*>(cur);
-#pragma unroll
-        for (int e = 0; e < 32; ++e) {
-          const float y = fmaf(pv[e], sc2, -mb2);
-          pv[e] = FZ_POLY_SEL(e) ? ex2_poly(y) : ex2(y);  // 3 MUFU : 1 polynomial
-        }
-#pragma unroll
-        for (int e = 0; e < 32; e += 4) { lf0 += pv[e]; lf1 += pv[e + 1]; lf2 += pv[e + 2]; lf3 += pv[e + 3]; }
-        uint32_t pk[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) pk[e] = pack_half2(pv[2 * e], pv[2 * e + 1]);
-        tmem_st_32x32b_x16(sbase + i * 16, pk);
-        if (i < 3) tmem_ld_wait();
-      }
-      tmem_st_wait();
-      tc_fence_before();
+    for (int A = 0; A < n_atoms; ++A) {
+      mbar_wait(&base_full[A & 1], (A >> 1) & 1);
+      mbar_wait(&ring_full[stage], phase);
+      wgmma_fence();
+      pv_mma<NCH>(o, desc_of(s_base + (A & 1) * kAtomBytes + wg * kHalfAtom), desc_of(s_ring + stage * p.ring_stage_bytes), A ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      release();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[b]);
-    }
-    dbg_acc[7] = clock64() - dbg_t0;  // end of the key loop
-    // ---- merge the two warpgroups' partial softmax (split-KV): O = (fA O_A + fB O_B) / (fA l_A + fB l_B) ----
-    const float l_own = (lf0 + lf1) + (lf2 + lf3);
-    xchg[(wg * 128 + row) * 2 + 0] = m_ref;
-    xchg[(wg * 128 + row) * 2 + 1] = l_own;
-    named_bar_sync(3, 256);
-    const float m_a = xchg[row * 2], l_a = xchg[row * 2 + 1];
-    const float m_b = xchg[(128 + row) * 2], l_b = xchg[(128 + row) * 2 + 1];
-    const bool has_b = n_tiles >= 2;
-    const float m_all = has_b ? fmaxf(m_a, m_b) : m_a;
-    float f_a = ex2((m_a - m_all) * sc2), f_b = has_b ? ex2((m_b - m_all) * sc2) : 0.f;
-    const float inv = 1.0f / (f_a * l_a + f_b * l_b);
-    f_a *= inv;
-    f_b *= inv;
-    FZ_TIMED(2, mbar_wait(o_full, 0));
-    tc_fence_after();
-    __half* orow = p.out + (static_cast<long long>(bf) * p.S_q + q0 + row) * p.ldo + head * p.d;
-    for (int c = wg * 16; c < p.d_pad; c += 32) {  // 16-column chunks alternate between the warpgroups
-      uint32_t r[16], r1[16];
-      tmem_ld_32x32b_x16(tmem_o + lane_addr + c, r);
-      if (has_b) tmem_ld_32x32b_x16(tmem_o + 64 + lane_addr + c, r1);
-      tmem_ld_wait();
-#pragma unroll
-      for (int e = 0; e < 16; e += 8) {
-        if (c + e < p.d) {
-          float o[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            o[i] = __uint_as_float(r[e + i]) * f_a;
-            if (has_b) o[i] = fmaf(__uint_as_float(r1[e + i]), f_b, o[i]);
-          }
-          uint4 v;
-          v.x = pack_half2(o[0], o[1]);
-          v.y = pack_half2(o[2], o[3]);
-          v.z = pack_half2(o[4], o[5]);
-          v.w = pack_half2(o[6], o[7]);
-          *reinterpret_cast<uint4*>(orow + c + e) = v;
-        }
-      }
-    }
-    if (dbg_on && lane == 0 && (warp == 0 || warp == 4)) {
-      const int base = warp == 0 ? 8 : 16;
-      for (int i = 0; i < 8; ++i) p.dbg[base + i] = dbg_acc[i];
-      p.dbg[base + 3] = clock64() - dbg_t0;
+      if (lane == 0) mbar_arrive(&base_empty[A & 1]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Hook-free text cross-attention at the 64x64-latent layers (attention_register.py:71-128 with q.shape[1] > 32**2: 77 keys, head dim 40).
-// 0.4 % of the FLOPs, but one CTA per 128 queries through the generic pipeline is a ~5 us dependent chain (Q load -> QK^T -> softmax ->
-// PV -> store) with one CTA per SM: 143 us per launch at BF = 16 against 13 us of HBM time (ncu, profiles/r02_shapes_v0.json).
-// Here a CTA keeps K (one atom) and V^T (two atoms) of its (frame, head) in shared memory and STREAMS a range of query tiles through a
-// two-deep pipeline: Q tiles arrive through a 2-stage TMA ring, S/P and O are double-buffered in TMEM (buffer b = 128 columns: scores /
-// packed fp16 probabilities in [0, 80), the O accumulator in [80, 128)), one warpgroup does softmax(t+1) before the epilogue of tile t, so
-// the tensor pipe, the MUFU and the global stores of consecutive tiles overlap.  256 TMEM columns and ~60 KB of shared memory: two CTAs
-// per SM.  Needs keys <= 80, d_pad <= 48, S_q % 128 == 0 (the SD-1.x r = 64 layers); everything else takes attn_plain_kernel.
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int kCrossVAtom = 8192;  // d_pad * 128 B <= 6144, rounded to the 1024-byte swizzle-atom alignment
-constexpr int kCrossSmem = 1024 + 2 * kAtomBytes + kAtomBytes + 2 * kCrossVAtom + 512;
-
-__global__ void __launch_bounds__(192, 2) attn_cross_kernel(const __grid_constant__ AttnParams p, int tiles_per_cta) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  pdl_launch_dependents();
-  const int head = blockIdx.y, bf = blockIdx.z;
-  const int q_tiles = p.S_q >> 7;
-  const int t0 = blockIdx.x * tiles_per_cta;
-  const int n = min(q_tiles, t0 + tiles_per_cta) - t0;
-
-  uint8_t* s_q = smem;                       // 2 x 16 KiB
-  uint8_t* s_k = s_q + 2 * kAtomBytes;       // 128 keys x 128 B (rows >= 77 zero-filled by TMA)
-  uint8_t* s_v = s_k + kAtomBytes;           // 2 x [d_pad][64 keys]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_v + 2 * kCrossVAtom);
-  uint64_t* q_full = bars;        // [2]
-  uint64_t* q_empty = bars + 2;   // [2]
-  uint64_t* kv_full = bars + 4;
-  uint64_t* s_full = bars + 5;    // [2]
-  uint64_t* p_full = bars + 7;    // [2]
-  uint64_t* o_full = bars + 9;    // [2]
-  uint64_t* o_free = bars + 11;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 13);
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&p.tmQ);
-    tma_prefetch_desc(&p.tmK2);
-    tma_prefetch_desc(&p.tmVt);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&q_full[b], 1);
-      mbar_init(&q_empty[b], 1);
-      mbar_init(&s_full[b], 1);
-      mbar_init(&p_full[b], 4);
-      mbar_init(&o_full[b], 1);
-      mbar_init(&o_free[b], 4);
-    }
-    mbar_init(kv_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == 5) tmem_alloc<256>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-  const int vt_atom_bytes = p.d_pad * 128;
-  const int src = p.src_index[0][bf];
-
-  if (n > 0) {
-    if (warp == 4) {
-      // =========================================== TMA producer ===========================================
-      if (elect_one()) {
-        mbar_expect_tx(kv_full, kAtomBytes + 2 * vt_atom_bytes);
-        tma_load_4d(s_k, &p.tmK2, kv_full, 0, head, 0, src);
-        tma_load_4d(s_v, &p.tmVt, kv_full, 0, 0, head, src);
-        tma_load_4d(s_v + kCrossVAtom, &p.tmVt, kv_full, 64, 0, head, src);
-        for (int i = 0; i < n; ++i) {
-          const int st = i & 1;
-          mbar_wait(&q_empty[st], ((i >> 1) & 1) ^ 1);
-          mbar_expect_tx(&q_full[st], kAtomBytes);
-          tma_load_4d(s_q + st * kAtomBytes, &p.tmQ, &q_full[st], 0, head, (t0 + i) << 7, bf);
-        }
-      }
-    } else if (warp == 5) {
-      // =========================================== MMA issuer ===========================================
-      const bool leader = elect_one();
-      const uint32_t idesc_s = umma_idesc_f16(128, 80);
-      const uint32_t idesc_o = umma_idesc_f16(128, p.d_pad);
-      const uint64_t desc_hi = umma_desc_k_sw128(0);
-      const uint32_t q_lo = (smem_u32(s_q) & 0x3FFFF) >> 4;
-      const uint32_t k_lo = (smem_u32(s_k) & 0x3FFFF) >> 4;
-      const uint32_t v_lo = (smem_u32(s_v) & 0x3FFFF) >> 4;
-      const int ksteps = (p.d + 15) >> 4;
-      auto issue_qk = [&](int i) {
-        const int b = i & 1;
-        mbar_wait(&q_full[b], (i >> 1) & 1);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t a_lo = q_lo + b * (kAtomBytes >> 4);
+  // ------------------------------ epilogue: O (registers) -> fp16 -> global ------------------------------
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (k < ksteps) umma_f16_ss(tmem_base + b * 128, desc_hi | (a_lo + 2 * k), desc_hi | (k_lo + 2 * k), idesc_s, k ? 1u : 0u);
-          umma_commit(&q_empty[b]);
-          umma_commit(&s_full[b]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(kv_full, 0);
-      tc_fence_after();
-      issue_qk(0);
-      if (n > 1) issue_qk(1);
-      for (int i = 0; i < n; ++i) {
-        const int b = i & 1;
-        mbar_wait(&p_full[b], (i >> 1) & 1);
-        mbar_wait(&o_free[b], ((i >> 1) & 1) ^ 1);  // the epilogue of tile i - 2 has read this O buffer
-        tc_fence_after();
-        if (leader) {
-          const uint32_t pa = tmem_base + b * 128, od = pa + 80;
+  for (int h = 0; h < 2; ++h) {
+    if (!row_ok[h]) continue;
+    const float o_scale = (!replace && !exact) ? (1.0f / l_run[h]) : 1.0f;
+    __half* orow = p.out + (static_cast<long long>(bf) * p.S_q + q[h]) * p.ldo + head * p.d;
 #pragma unroll
-          for (int k = 0; k < 5; ++k) {
-            const uint64_t bdesc = desc_hi | (v_lo + (k >> 2) * (kCrossVAtom >> 4) + 2 * (k & 3));
-            umma_f16_ts(od, pa + k * 8, bdesc, idesc_o, k ? 1u : 0u);
-          }
-          umma_commit(&o_full[b]);
-        }
-        __syncwarp();
-        if (i + 2 < n) issue_qk(i + 2);  // executes behind PV(i) on the tensor pipe: reuses the S/P columns PV(i) has just read
-      }
-    } else {
-      // =========================================== softmax + epilogue warpgroup ===========================================
-      const int row = warp * 32 + lane;
-      const uint32_t lane_addr = static_cast<uint32_t>(warp * 32) << 16;
-      const float sc2 = p.scale_log2;
-      const int keys = p.keys_per_slot;
-      float l_sum[2] = {0.f, 0.f};
-      for (int j = 0; j <= n; ++j) {
-        if (j < n) {
-          const int b = j & 1;
-          mbar_wait(&s_full[b], (j >> 1) & 1);
-          tc_fence_after();
-          const uint32_t sb = tmem_base + lane_addr + b * 128;
-          uint32_t r0[32], r1[32], r2[16];
-          tmem_ld_32x32b_x32(sb, r0);
-          tmem_ld_32x32b_x32(sb + 32, r1);
-          tmem_ld_32x32b_x16(sb + 64, r2);
-          tmem_ld_wait();
-          float s[80];
-#pragma unroll
-          for (int e = 0; e < 32; ++e) { s[e] = __uint_as_float(r0[e]); s[32 + e] = __uint_as_float(r1[e]); }
-#pragma unroll
-          for (int e = 0; e < 16; ++e) s[64 + e] = __uint_as_float(r2[e]);
-#pragma unroll
-          for (int e = 64; e < 80; ++e)
-            if (e >= keys) s[e] = -INFINITY;
-          if (keys < 64) {
-#pragma unroll
-            for (int e = 0; e < 64; ++e)
-              if (e >= keys) s[e] = -INFINITY;
-          }
-          float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-          for (int e = 0; e < 80; e += 4) {
-            m0 = fmaxf(m0, s[e]); m1 = fmaxf(m1, s[e + 1]); m2 = fmaxf(m2, s[e + 2]); m3 = fmaxf(m3, s[e + 3]);
-          }
-          const float mb = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)) * sc2;
-          float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-          for (int e = 0; e < 80; e += 4) {
-            s[e] = ex2(fmaf(s[e], sc2, -mb)); s[e + 1] = ex2(fmaf(s[e + 1], sc2, -mb));
-            s[e + 2] = ex2(fmaf(s[e + 2], sc2, -mb)); s[e + 3] = ex2(fmaf(s[e + 3], sc2, -mb));
-            a0 += s[e]; a1 += s[e + 1]; a2 += s[e + 2]; a3 += s[e + 3];
-          }
-          l_sum[b] = (a0 + a1) + (a2 + a3);
-          uint32_t pk0[32], pk1[16];
-#pragma unroll
-          for (int e = 0; e < 32; ++e) pk0[e] = pack_half2(s[2 * e], s[2 * e + 1]);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) pk1[e] = pack_half2(s[64 + 2 * e], s[64 + 2 * e + 1]);
-#pragma unroll
-          for (int e = 8; e < 16; ++e) pk1[e] = 0u;
-          tmem_st_32x32b_x32(sb, pk0);
-          tmem_st_32x32b_x16(sb + 32, pk1);
-          tmem_st_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&p_full[b]);
-        }
-        if (j >= 1) {
-          const int i = j - 1, b = i & 1;
-          mbar_wait(&o_full[b], (i >> 1) & 1);
-          tc_fence_after();
-          const uint32_t ob = tmem_base + lane_addr + b * 128 + 80;
-          uint32_t o0[32], o1[16];
-          tmem_ld_32x32b_x32(ob, o0);
-          tmem_ld_32x32b_x16(ob + 32, o1);
-          tmem_ld_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&o_free[b]);
-          const float inv = 1.0f / l_sum[b];
-          __half* orow = p.out + (static_cast<long long>(bf) * p.S_q + ((t0 + i) << 7) + row) * p.ldo + head * p.d;
-#pragma unroll
-          for (int c = 0; c < 48; c += 8) {
-            if (c < p.d) {
-              uint4 v;
-              if (c < 32) {
-                v.x = pack_half2(__uint_as_float(o0[c + 0]) * inv, __uint_as_float(o0[c + 1]) * inv);
-                v.y = pack_half2(__uint_as_float(o0[c + 2]) * inv, __uint_as_float(o0[c + 3]) * inv);
-                v.z = pack_half2(__uint_as_float(o0[c + 4]) * inv, __uint_as_float(o0[c + 5]) * inv);
-                v.w = pack_half2(__uint_as_float(o0[c + 6]) * inv, __uint_as_float(o0[c + 7]) * inv);
-              } else {
-                v.x = pack_half2(__uint_as_float(o1[c - 32 + 0]) * inv, __uint_as_float(o1[c - 32 + 1]) * inv);
-                v.y = pack_half2(__uint_as_float(o1[c - 32 + 2]) * inv, __uint_as_float(o1[c - 32 + 3]) * inv);
-                v.z = pack_half2(__uint_as_float(o1[c - 32 + 4]) * inv, __uint_as_float(o1[c - 32 + 5]) * inv);
-                v.w = pack_half2(__uint_as_float(o1[c - 32 + 6]) * inv, __uint_as_float(o1[c - 32 + 7]) * inv);
-              }
-              *reinterpret_cast<uint4*>(orow + c) = v;
-            }
-          }
-        }
-      }
+    for (int i = 0; i < 8 * NCH; ++i) {
+      const int c = 8 * i + c_base;
+      if (c < p.d) *reinterpret_cast<uint32_t*>(orow + c) = pack_half2(o[4 * i + 2 * h] * o_scale, o[4 * i + 2 * h + 1] * o_scale);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
-  }
+  if (row_mode == FZ_ATTN_STORE && st == 0) tma_store_wait_all<0>();
 }
 
 }  // namespace fz
@@ -1242,7 +482,7 @@ static int encode_cache_map(CUtensorMap* tm, const void* base, int keys_ld_slot,
   // cache slab [Fc, heads, S_q, row_ld] fp16; a row holds n_slots runs of keys_ld_slot keys (self) or one run (cross)
   uint64_t dims[5] = {(uint64_t)keys_ld_slot, (uint64_t)n_slots, (uint64_t)S_q, (uint64_t)heads, (uint64_t)Fc};
   uint64_t strides[4] = {(uint64_t)keys_ld_slot, (uint64_t)row_ld, (uint64_t)row_ld * S_q, (uint64_t)row_ld * S_q * heads};
-  uint32_t box[5] = {64, 1, 128, 1, 1};
+  uint32_t box[5] = {64, 1, 64, 1, 1};
   return encode_tmap_f16(tm, base, 5, dims, strides, box, true);
 }
 
@@ -1256,7 +496,7 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.S_q = a->S_q; p.keys_per_slot = a->keys_per_slot; p.n_slots = a->n_slots;
-  p.d = a->d; p.d_pad = (a->d + 15) / 16 * 16; p.nd = (a->d + 63) / 64;
+  p.d = a->d; p.nd = (a->d + 63) / 64;
   p.heads = a->heads; p.F = a->F; p.BF = a->BF;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   for (int s = 0; s < a->n_slots; ++s)
@@ -1266,8 +506,8 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   p.base_rows = static_cast<const __half*>(a->base); p.base_ld = a->cache_ld;
   p.xedit = a->xedit; p.mask = a->mask;
   p.out = static_cast<__half*>(a->out); p.ldo = a->ldo;
-  p.dbg = static_cast<long long*>(a->dbg);
   p.causal = a->causal;
+  p.masked = a->causal || a->keys_per_slot % 64 != 0;
   if (a->causal) FZ_CHECK_ARG(a->n_slots == 1 && a->row_mode == FZ_ATTN_NONE && !a->acc, "fz_attention: causal masking needs one slot and no controller hook");
   const int Fc = a->BF - a->edit_bf_start;
   if (a->row_mode == FZ_ATTN_STORE) FZ_CHECK_ARG(a->store, "fz_attention: STORE needs a cache slab");
@@ -1291,45 +531,9 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   {
     uint64_t dims[4] = {(uint64_t)a->keys_per_slot, (uint64_t)a->d, (uint64_t)a->heads, (uint64_t)a->n_src};
     uint64_t strides[3] = {(uint64_t)a->vt_ld, (uint64_t)a->vt_ld * a->d, (uint64_t)a->vt_ld * a->d * a->heads};
-    uint32_t box[4] = {64, (uint32_t)p.d_pad, 1, 1};
+    uint32_t box[4] = {64, (uint32_t)(64 * p.nd), 1, 1};  // rows beyond d: zero fill (fixed-shape PV wgmma)
     if (int rc = encode_tmap_f16(&p.tmVt, a->vt, 4, dims, strides, box, true)) return rc;
   }
-  // rows without any controller hook and a small head dim take the TMEM-resident-P kernel
-  const bool plain = !a->causal && (a->row_mode == FZ_ATTN_NONE || a->edit_bf_start >= a->BF) && !a->acc && a->d <= 64 &&
-                     (a->keys_per_slot % 128 == 0 || a->n_slots == 1) && a->S_q % 128 == 0;
-  if (plain) {
-    uint64_t dims[4] = {(uint64_t)a->d, (uint64_t)a->heads, (uint64_t)a->keys_per_slot, (uint64_t)a->n_src};
-    uint64_t strides[3] = {(uint64_t)a->d, (uint64_t)a->ldk, (uint64_t)a->ldk * a->keys_per_slot};
-    uint32_t box[4] = {64, 1, 128, 1};
-    if (int rc = encode_tmap_f16(&p.tmK2, a->k, 4, dims, strides, box, true)) return rc;
-    if (a->n_slots == 1 && a->keys_per_slot <= 80 && p.d_pad <= 48) {
-      // text cross-attention of the un-hooked layers: the streaming kernel (K / V^T resident, query tiles pipelined, 2 CTAs per SM)
-      static bool configured_cross = false;
-      if (!configured_cross) {
-        FZ_CUDA(cudaFuncSetAttribute(attn_cross_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCrossSmem));
-        configured_cross = true;
-      }
-      const int q_tiles = a->S_q / 128;
-      int splits = std::max(1, std::min(q_tiles, (296 + a->heads * a->BF - 1) / (a->heads * a->BF)));
-      const int tiles_per_cta = (q_tiles + splits - 1) / splits;
-      splits = (q_tiles + tiles_per_cta - 1) / tiles_per_cta;
-      FZ_CUDA(launch_pdl(attn_cross_kernel, dim3(splits, a->heads, a->BF), dim3(192), kCrossSmem, stream, p, tiles_per_cta));
-      FZ_CUDA(cudaGetLastError());
-      return FZ_OK;
-    }
-    static bool configured_plain = false;
-    if (!configured_plain) {
-      FZ_CUDA(cudaFuncSetAttribute(attn_plain_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPlainSmem));
-      FZ_CUDA(cudaFuncSetAttribute(attn_plain_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPlainSmem));
-      configured_plain = true;
-    }
-    dim3 grid(a->S_q / 128, a->heads, a->BF);
-    if (a->keys_per_slot % 128 == 0) FZ_CUDA(launch_pdl(attn_plain_kernel<false>, grid, dim3(320), kPlainSmem, stream, p));
-    else FZ_CUDA(launch_pdl(attn_plain_kernel<true>, grid, dim3(320), kPlainSmem, stream, p));
-    FZ_CUDA(cudaGetLastError());
-    return FZ_OK;
-  }
-  p.tmK2 = p.tmK;
   // cache geometry: a row of the slab is n_slots * keys_ld_slot wide, keys_ld_slot = cache_ld / n_slots
   if (a->store) {
     if (int rc = encode_cache_map(&p.tmStore, a->store, (int)(a->cache_ld / a->n_slots), a->n_slots, a->S_q, a->heads, Fc, a->cache_ld)) return rc;
@@ -1341,23 +545,25 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   } else {
     p.tmBase = p.tmQ;
   }
-  // shared memory plan
-  const int stage_bytes = std::max(8192, (p.d_pad * 128 + 1023) / 1024 * 1024);
-  const int fixed = p.nd * kAtomBytes + 4 * kAtomBytes + (a->row_mode == FZ_ATTN_BLEND ? 2 * kAtomBytes : 0) + 1024 + 3072;
-  int stages = 10;
-  while (stages > 3 && fixed + stages * stage_bytes > 225 * 1024) --stages;
+  // shared memory plan: Q + ring + 4 half P tiles (+ 2 base tiles) + barriers
+  const bool has_base = a->row_mode == FZ_ATTN_REPLACE || a->row_mode == FZ_ATTN_BLEND;
+  const int stage_bytes = p.nd * 64 * 128;
+  const int fixed = p.nd * kAtomBytes + 4 * kHalfAtom + (has_base ? 2 * kAtomBytes : 0) + 1024 + 512;
+  int stages = kMaxStages;
+  while (stages > 2 && fixed + stages * stage_bytes > 227 * 1024) --stages;
   FZ_CHECK_ARG(fixed + stages * stage_bytes <= 227 * 1024, "fz_attention: shared memory plan does not fit (d=%d)", a->d);
   p.ring_stages = stages; p.ring_stage_bytes = stage_bytes;
   const int smem = fixed + stages * stage_bytes;
-  static int configured = 0;
-  if (smem > configured) {
-    FZ_CUDA(cudaFuncSetAttribute(attn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    FZ_CUDA(cudaFuncSetAttribute(attn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured = smem;
+  static bool configured = false;
+  if (!configured) {
+    FZ_CUDA(cudaFuncSetAttribute(attn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    FZ_CUDA(cudaFuncSetAttribute(attn_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    FZ_CUDA(cudaFuncSetAttribute(attn_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    configured = true;
   }
   dim3 grid((a->S_q + 127) / 128, a->heads, a->BF);
-  if (a->keys_per_slot % 64 == 0 && !a->causal) FZ_CUDA(launch_pdl(attn_kernel<false>, grid, dim3(320), smem, stream, p));
-  else FZ_CUDA(launch_pdl(attn_kernel<true>, grid, dim3(320), smem, stream, p));
+  auto kernel = p.nd == 1 ? attn_kernel<1> : p.nd == 2 ? attn_kernel<2> : attn_kernel<3>;
+  FZ_CUDA(launch_pdl(kernel, grid, dim3(288), smem, stream, p));
   FZ_CUDA(cudaGetLastError());
   return FZ_OK;
 }

@@ -106,8 +106,8 @@ extern "C" int fz_device_check(void) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10) {
-    fz::set_error("libfatezero_b200 needs an sm_100-class GPU (found sm_%d%d)", major, minor);
+  if (major != 9 || minor != 0) {
+    fz::set_error("libfatezero_b200 is built for sm_90a (H100) and needs an sm_90 GPU (found sm_%d%d)", major, minor);
     return FZ_ERR_INVALID;
   }
   return FZ_OK;

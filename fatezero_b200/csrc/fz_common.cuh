@@ -1,7 +1,7 @@
-// fz_common.cuh — sm_100a building blocks shared by the FateZero-B200 kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), UMMA descriptors, host tensor-map encode.
-// Hand-written inline PTX; descriptor bit layouts follow the PTX ISA tcgen05 "shared memory descriptor" and
-// "instruction descriptor" tables (K-major, SWIZZLE_128B, fp16 inputs, fp32 accumulate).
+// fz_common.cuh — sm_90a building blocks shared by the FateZero kernels:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors (fz_wgmma.cuh has the MMA wrappers), host tensor-map encode.
+// Hand-written inline PTX; descriptor bit layouts follow the PTX ISA wgmma "matrix descriptor" table
+// (K-major, SWIZZLE_128B, fp16 inputs, fp32 accumulate).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -46,7 +46,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast
 
 // ---- programmatic dependent launch (PDL) --------------------------------------------------------------------------
 // A UNet step is ~1170 short dependent launches; with programmatic stream serialisation the next kernel's CTAs are scheduled
-// while the current one drains and run their prologue (barrier init, TMEM allocation, descriptor prefetch) up to pdl_wait(),
+// while the current one drains and run their prologue (barrier init, descriptor prefetch) up to pdl_wait(),
 // which returns once the preceding kernel has completed and its writes are visible.  Every kernel launched through launch_pdl
 // calls pdl_launch_dependents() first and pdl_wait() before its first global-memory access (read OR write).
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -89,30 +89,16 @@ __device__ __forceinline__ uint64_t global_timer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// slow path kept out of line: the inlined fast path is one try_wait + branch (the MMA-issuing warps execute thousands of waits)
-static __device__ __noinline__ void mbar_wait_slow(uint32_t bar_addr, uint32_t parity) {
-  const uint64_t t0 = global_timer_ns();
-  uint32_t spins = 0;
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-        : "=r"(ok)
-        : "r"(bar_addr), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if ((++spins & 0x3ff) == 0 && global_timer_ns() - t0 > FZ_MBAR_TIMEOUT_NS) {
-      printf("fz: mbarrier wait timed out (block %d,%d,%d thread %d bar 0x%x parity %u)\n", blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x,
-             bar_addr, parity);
-      __trap();
-    }
-  }
-}
+// Entirely inline: any function call in a kernel that issues wgmma (an out-of-line slow path, printf) makes ptxas serialise its wgmma
+// instructions, so a timeout traps without a diagnostic message.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (!mbar_try_wait(bar, parity)) mbar_wait_slow(smem_u32(bar), parity);
+  if (mbar_try_wait(bar, parity)) return;
+  const uint64_t t0 = global_timer_ns();
+  while (!mbar_try_wait(bar, parity))
+    if (global_timer_ns() - t0 > FZ_MBAR_TIMEOUT_NS) __trap();
 }
 
-// generic-proxy writes (st.shared) -> visible to the async proxy (TMA store / tcgen05.mma operand reads)
+// generic-proxy writes (st.shared) -> visible to the async proxy (TMA store / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- TMA -------------------------------------------------------------------------------------------------------
@@ -175,113 +161,21 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---- tcgen05 ---------------------------------------------------------------------------------------------------
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; fp16 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (M=128 rows = TMEM lanes, K fp16 elements packed two per 32-bit column) is read
-// from tensor memory, e.g. softmax probabilities written by tcgen05.st over the score columns they were computed from.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 32 columns of fp32: thread (lane l of warp w) receives TMEM lane 32*(w%4)+l, columns [col, col+32).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM: lane i of the warp writes 32 consecutive 32-bit columns of TMEM lane (warp % 4) * 32 + i
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- UMMA descriptors --------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major operand tile stored as rows of 128 bytes (64 fp16) with the 128-byte swizzle
-// (exactly what a TMA box {64, rows} with CU_TENSOR_MAP_SWIZZLE_128B writes):
+// ---- wgmma operand descriptors ----------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (sm_90 wgmma), K-major operand tile stored as rows of 128 bytes (64 fp16) with the 128-byte
+// swizzle (exactly what a TMA box {64, rows} with CU_TENSOR_MAP_SWIZZLE_128B writes; tiles 1024-byte aligned):
 //   bits [ 0,14) start address >> 4        bits [16,30) leading-dim byte offset >> 4 (ignored for swizzled K-major; 1)
-//   bits [32,46) stride-dim byte offset >> 4 = 1024 B between 8-row groups
-//   bits [46,48) descriptor version = 1 (sm_100)          bits [61,64) layout type = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+//   bits [32,46) stride-dim byte offset >> 4 = 1024 B between 8-row groups          bits [62,64) layout type = 1 (SWIZZLE_128B)
+// The k-th 16-element K step of a tile starts 32 bytes further: add 2 * k to the descriptor's low word.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor (.kind::f16): c_format F32 (bits 4-5 = 1), a/b format F16 (0), K-major A and B (bits 15,16 = 0),
-// N>>3 at bits [17,23), M>>4 at bits [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t m, uint32_t n) {
-  return (1u << 4) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 #endif  // __CUDACC__
 

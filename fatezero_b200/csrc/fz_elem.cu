@@ -1,7 +1,7 @@
 // fz_elem.cu — HBM-bound kernels of the UNet step: GroupNorm (joint-frame statistics), LayerNorm, nearest upsample,
 // channel concat, input im2col / output temporal conv, time embedding, temporal attention, CFG + DDIM + latent blend,
 // and the cross-attention blend mask.  All activations are fp16 NHWC ([B*F, H*W, C] == token-major), statistics fp32/fp64,
-// 16-byte vector loads/stores, grids sized to cover the 148 SMs.
+// 16-byte vector loads/stores, grids sized to cover the 132 SMs.
 #include "fz_common.cuh"
 
 #include <algorithm>
@@ -17,7 +17,7 @@ static inline int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -1050,7 +1050,7 @@ extern "C" int fz_embed_tokens_f16(const float* tok, const float* pos, const lon
 }
 extern "C" int fz_quick_gelu_f16(void* x, long long n, cudaStream_t stream) {
   FZ_CHECK_ARG(x && n > 0, "fz_quick_gelu: bad args");
-  fz::quick_gelu_kernel<<<static_cast<int>(std::min<long long>((n + 255) / 256, 148 * 8)), 256, 0, stream>>>(static_cast<__half*>(x), n);
+  fz::quick_gelu_kernel<<<static_cast<int>(std::min<long long>((n + 255) / 256, 132 * 8)), 256, 0, stream>>>(static_cast<__half*>(x), n);
   FZ_CUDA(cudaGetLastError());
   return FZ_OK;
 }
@@ -1058,7 +1058,7 @@ extern "C" int fz_quick_gelu_f16(void* x, long long n, cudaStream_t stream) {
 // ---------------------------------------------------------------------------------------------------------------
 // Row softmax in place: x[r, :n] <- softmax(scale * x[r, :n]) (fp32 math, fp16 storage).  The VAE's single-head 512-wide mid-block
 // attention (diffusers AttentionBlock: stable_diffusion.py:297-319 decode path) runs as GEMM -> this -> GEMM: its head dim exceeds what
-// the fused attention kernels hold in TMEM.  One warp per row.
+// the fused attention kernel holds in registers (d <= 192).  One warp per row.
 // ---------------------------------------------------------------------------------------------------------------
 namespace fz {
 __global__ void __launch_bounds__(256) softmax_rows_kernel(__half* __restrict__ x, long long rows, int n, long long ld, float scale_log2) {

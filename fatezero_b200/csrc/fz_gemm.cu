@@ -1,4 +1,4 @@
-// fz_gemm.cu — the "tap-GEMM": one persistent, warp-specialised tcgen05 kernel that serves every dense contraction of the
+// fz_gemm.cu — the "tap-GEMM": one persistent, warp-specialised wgmma kernel that serves every dense contraction of the
 // UNet step except attention:
 //     D[M, N] = sum_{tap} A_tap[M, K] * W_tap[N, K]^T   (+ bias, + per-batch time-embedding row, + residual, GEGLU, V^T store)
 //   * nn.Linear / 1x1 conv ............ 1 tap, A = [M, K] row-major tokens
@@ -8,13 +8,13 @@
 // Reference ops replaced: models/resnet.py:57-80 (PseudoConv3d.forward), models/lora.py:46-54, nn.Linear call sites of
 // prompt_attention/attention_register.py:81,99-100,124,156-160,214 and diffusers FeedForward/GEGLU (models/attention.py:320).
 //
-// Structure (per CTA, 320 threads, 1 CTA / SM, grid = min(#tiles, #SMs), static round-robin tile schedule):
-//   warp 0 : TMA producer   — A box {64ch, rows} + W box {64ch, BLOCK_N} per stage, SWIZZLE_128B, mbarrier complete_tx
-//   warp 1 : MMA issuer     — tcgen05.mma.cta_group::1.kind::f16  M=128 x N=BLOCK_N x K=16, fp32 accumulators in TMEM,
-//                             double-buffered accumulators (2 x BLOCK_N columns) so the epilogue overlaps the next tile
-//   warps 2-9 : epilogue    — tcgen05.ld 32x32b -> registers -> fused epilogue -> 16-byte global stores (two warps per TMEM
-//                             lane quadrant, alternating 32-column chunks)
+// Structure (per CTA, 384 threads = 3 warpgroups, 1 CTA / SM, grid = min(#tiles, #SMs), static round-robin tile schedule):
+//   warpgroup 2    : TMA producer — A box {64ch, rows} + W box {64ch, BLOCK_N} per stage, SWIZZLE_128B, mbarrier complete_tx
+//   warpgroups 0-1 : consumers   — wgmma m64 x N=BLOCK_N x k16 on rows [64 wg, 64 wg + 64) of the 128-row tile, fp32 accumulators
+//                                  in registers, fused epilogue straight from the accumulator fragment while the producer already
+//                                  fills the ring with the next tile's operands
 #include "fz_common.cuh"
+#include "fz_wgmma.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -33,15 +33,10 @@ constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KiB
 struct TapGemmParams {
   CUtensorMap tmA;
   CUtensorMap tmB;
-  CUtensorMap tmC;    // output [M, N] as (cols, rows), box {32 cols, 32 rows}, SWIZZLE_64B (epilogue TMA stores)
-  CUtensorMap tmC16;  // same output with box {16 cols, 32 rows}, no swizzle (GEGLU epilogue with 16-column chunks)
   CUtensorMap tmR[2]; // skip tensors [M, N] folded into the accumulator as extra k-blocks: box {64 cols, 128 rows}
   CUtensorMap tmE;    // identity blocks E[j][n][k] = (n == 64 j + k): (k : 64, n : 256, j : 4), box {64, BLOCK_N, 1}
-  CUtensorMap tmVt;   // V^T output [BF * heads * d rows, vt_ld] as (s, row), box {32 s, 32 rows}: transposed chunks leave through smem + TMA
-  int vt_tma;         // 1 = the V^T columns take the staged TMA path (vt_S % 32 == 0), 0 = per-element stores
   int n_res;          // number of folded skip tensors (0..2); the epilogue then sees residual == residual2 == null
   int res_kblocks;    // ceil(BLOCK_N / 64) extra k-blocks per folded skip tensor
-  int use_tma_store;  // 0 = direct 16-byte stores (fallback for odd geometries)
   int a_rank;         // 2..5
   int M, N;           // valid output rows / columns (for GEGLU: N = number of OUTPUT columns = half the GEMM columns)
   int rows_per_tile;  // <= 128; tile t covers output rows [t*rows_per_tile, ...)
@@ -72,18 +67,14 @@ struct TapGemmCfg {
   static constexpr int kBTileBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kBTilePad = (kBTileBytes + 1023) / 1024 * 1024;
   static constexpr int kStageBytes = kATileBytes + kBTilePad;
-  static constexpr int kEpiBytes = 8 * 2 * 2048;  // 8 epilogue warps x 2 staging slots of 32 rows x 64 B
-  static constexpr int kStagesRaw = (227 * 1024 - kEpiBytes - 1280) / kStageBytes;
+  static constexpr int kStagesRaw = (227 * 1024 - 1280) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kTmemCols = (2 * BLOCK_N <= 32) ? 32 : (2 * BLOCK_N <= 64) ? 64 : (2 * BLOCK_N <= 128) ? 128 : (2 * BLOCK_N <= 256) ? 256 : 512;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 // exact-erf GELU (F.gelu default).  erf via Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7, far below the fp16 output rounding):
-// 1 MUFU.RCP + 1 MUFU.EX2 + 8 FMA instead of the ~40-instruction erff() — the GEGLU epilogue was XU/ALU-bound (ncu: 24 % tensor pipe).
+// 1 MUFU.RCP + 1 MUFU.EX2 + 8 FMA instead of the ~40-instruction erff().
 __device__ __forceinline__ float gelu_erf(float x) {
-  // single-instruction MUFU forms: __frcp_rn / exp2f expand to IEEE-exact sequences (~10 extra instructions each) and made the GEGLU
-  // epilogue latency-bound (measured 4900 cycles per 32x32 chunk, 84 % of the epilogue warp's time)
   const float z = fabsf(x) * 0.70710678118654752f;
   float t, e;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.3275911f, z, 1.0f)));
@@ -96,75 +87,53 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return 0.5f * x * (1.0f + copysignf(erf_abs, x));
 }
 
-__device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
-  __half2 h = __floats2half2_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&h);
+// one output element of the row-major / V^T epilogue (right-edge columns and the V^T part; the paired fast path is inlined below)
+__device__ __forceinline__ void epi_store1(const TapGemmParams& p, long long m, int col, float v, const float* gb) {
+  if (p.bias) v += __ldg(p.bias + col);
+  if (col >= p.vt_col_start) {
+    const long long bf = m / p.vt_S;
+    const int s = static_cast<int>(m % p.vt_S);
+    const int cv = col - p.vt_col_start;
+    p.out_vt[((bf * p.vt_heads + cv / p.vt_d) * p.vt_d + cv % p.vt_d) * p.vt_ld + s] = __float2half_rn(v);
+  } else {
+    if (gb) v += __ldg(gb + col);
+    if (p.residual) v += __half2float(p.residual[m * p.ldr + col]);
+    if (p.residual2) v += __half2float(p.residual2[m * p.ldr2 + col]);
+    p.out[m * p.ldo + col] = __float2half_rn(v);
+  }
 }
 
-// Optional in-kernel cycle accounting (compile with -DFZ_GEMM_PROFILE, read with fz_debug_gemm_counters): CTA 0 only.
-//  [0] epilogue warp 2: loop total  [1] wait tfull  [2] TMEM load  [3] math  [4] wait for a free staging slot  [5] stage + TMA store
-//  [6] chunks  [7] tiles   [8] MMA thread: total  [9] wait tempty  [10] wait full   [12] producer: total  [13] wait empty
-__device__ long long g_gemm_dbg[16];
-#ifdef FZ_GEMM_PROFILE
-#define GP_NOW() clock64()
-#define GP_ADD(slot, expr) do { if (gp_on) gp[slot] += (expr); } while (0)
-#else
-#define GP_NOW() 0LL
-#define GP_ADD(slot, expr) do { } while (0)
-#endif
-
-// EPI_GROUPS = epilogue warps per TMEM lane quadrant: 2 (320 threads) for every row-major epilogue; 4 (576 threads, 16-column chunks so that
-// the kernel fits the smaller register budget) for the GEGLU epilogue, which is ALU-bound: it was 3x the mainloop with two warps per scheduler.
-template <int BLOCK_N, int EPI_GROUPS = 2>
-__global__ void __launch_bounds__(64 + 128 * EPI_GROUPS, 1) tapgemm_kernel(const __grid_constant__ TapGemmParams p) {
+template <int BLOCK_N>
+__global__ void __launch_bounds__(384, 1) tapgemm_kernel(const __grid_constant__ TapGemmParams p) {
   using Cfg = TapGemmCfg<BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* epi_smem = smem + Cfg::kStages * Cfg::kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_smem + Cfg::kEpiBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* tfull = bars + 2 * Cfg::kStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   pdl_launch_dependents();
-#ifdef FZ_GEMM_PROFILE
-  const bool gp_on = blockIdx.x == 0;
-  long long gp[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-#endif
-  const int lane = threadIdx.x & 31;
   const int num_tiles = p.m_tiles * p.n_tiles;
   const int k_iters = p.num_taps * p.k_blocks + p.n_res * p.res_kblocks;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
-    if (p.use_tma_store) tma_prefetch_desc(&p.tmC);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull[b], 1);
-      mbar_init(&tempty[b], 4 * EPI_GROUPS);
+      mbar_init(&empty[s], 8);  // one arrive per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();  // everything above overlapped the previous kernel's tail; operands / outputs are touched only from here on
 
-  if (warp == 0) {
+  if (wg == 2) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    if (threadIdx.x == 256) {
       int stage = 0;
       uint32_t phase = 0;
-      const long long gp_t0 = GP_NOW();
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int mt = tile / p.n_tiles, nt = tile % p.n_tiles;
         int rem = mt * p.rows_per_tile;
@@ -178,9 +147,7 @@ __global__ void __launch_bounds__(64 + 128 * EPI_GROUPS, 1) tapgemm_kernel(const
           const int c1 = base[1] + p.tap_off[tap][1], c2 = base[2] + p.tap_off[tap][2];
           const int c3 = base[3] + p.tap_off[tap][3], c4 = base[4] + p.tap_off[tap][4];
           for (int kb = 0; kb < p.k_blocks; ++kb) {
-            const long long gp_a = GP_NOW();
             mbar_wait(&empty[stage], phase ^ 1);
-            GP_ADD(13, GP_NOW() - gp_a);
             uint8_t* sa = smem + stage * Cfg::kStageBytes;
             uint8_t* sb = sa + kATileBytes;
             mbar_expect_tx(&full[stage], p.a_box_bytes + Cfg::kBTileBytes);
@@ -196,9 +163,8 @@ __global__ void __launch_bounds__(64 + 128 * EPI_GROUPS, 1) tapgemm_kernel(const
           }
         }
         // Skip connections ride the same pipeline as extra k-blocks: D += R[:, n0 + 64 j ...] * E_j^T with E_j a 0/1 selection block
-        // (exact: fp16 x 1.0 accumulated in fp32 after the last tap, the same order as an epilogue add).  The epilogue of a
-        // K = 320 linear used to wait ~1 us of exposed global-load latency per 32-column chunk for the skip tensor
-        // (65536 x 320 x 320 + skip: 40 us against 21 us without); here the loads are prefetched by the TMA ring like any operand.
+        // (exact: fp16 x 1.0 accumulated in fp32 after the last tap, the same order as an epilogue add), so the skip tensor is
+        // prefetched by the TMA ring like any operand instead of being waited for in the epilogue.
         for (int r = 0; r < p.n_res; ++r) {
           for (int j = 0; j < p.res_kblocks; ++j) {
             mbar_wait(&empty[stage], phase ^ 1);
@@ -211,433 +177,91 @@ __global__ void __launch_bounds__(64 + 128 * EPI_GROUPS, 1) tapgemm_kernel(const
           }
         }
       }
-#ifdef FZ_GEMM_PROFILE
-      if (gp_on) { g_gemm_dbg[12] = GP_NOW() - gp_t0; g_gemm_dbg[13] = gp[13]; }
-#endif
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_f16(kBlockM, BLOCK_N);
-      const uint64_t desc_hi = umma_desc_k_sw128(0);  // constant descriptor fields; only the 14-bit start address varies
-      const uint32_t smem_lo0 = (smem_u32(smem) & 0x3FFFF) >> 4;
-      int stage = 0;
-      uint32_t phase = 0;
-      int local = 0;
-      const long long gp_m0 = GP_NOW();
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-        const int buf = local & 1;
-        const uint32_t use = static_cast<uint32_t>(local >> 1);
-        const long long gp_a = GP_NOW();
-        mbar_wait(&tempty[buf], (use & 1) ^ 1);
-        GP_ADD(9, GP_NOW() - gp_a);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * BLOCK_N;
-        for (int it = 0; it < k_iters; ++it) {
-          const long long gp_b = GP_NOW();
-          mbar_wait(&full[stage], phase);
-          GP_ADD(10, GP_NOW() - gp_b);
-          tc_fence_after();
-          const uint32_t a_lo = smem_lo0 + stage * (Cfg::kStageBytes >> 4);
-          const uint32_t b_lo = a_lo + (kATileBytes >> 4);
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) {
-            umma_f16_ss(d_tmem, desc_hi | (a_lo + 2 * k), desc_hi | (b_lo + 2 * k), idesc, (it | k) ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull[buf]);
-      }
-#ifdef FZ_GEMM_PROFILE
-      if (gp_on) { g_gemm_dbg[8] = GP_NOW() - gp_m0; g_gemm_dbg[9] = gp[9]; g_gemm_dbg[10] = gp[10]; }
-#endif
-    }
-  } else {
-    // ===================== epilogue warps =====================
-    // Straight-line fast path per 32-column chunk (all option tests are warp-uniform and hoisted out of the element loops):
-    // the v0 epilogue spent ~46 instructions per output element on per-element bound / option branches (ncu: 7 % tensor pipe
-    // on K=320 GEMMs); edge tiles fall back to the generic masked path.
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may read
-    const int half = (warp - 2) >> 2;  // the EPI_GROUPS warps of a quadrant take alternating column chunks
-    const int row_in_tile = quad * 32 + lane;
-    // Coalesced output path: each warp stages its 32 rows x 32 columns (64 B rows, 64-byte swizzle => conflict-free 16-byte
-    // st.shared) and one lane issues a TMA store; direct per-row 16-byte stores touch 32 lines per instruction and made the
-    // epilogue LSU-bound (~2.4 us per 128x160 tile).
-    constexpr int kSlotBytes = (EPI_GROUPS == 4) ? 1024 : 2048;  // 32 rows x (16 | 32) fp16 columns
-    uint8_t* my_epi = epi_smem + (warp - 2) * 2 * kSlotBytes;
-    uint32_t epi_count = 0;
-    auto store_chunk32 = [&](const uint4 (&o)[4], long long m_row, int col, int m_warp0, uint8_t* acquired) {
-      if (p.use_tma_store) {
-        uint8_t* slot = acquired;
-        const long long gp_a = GP_NOW();
-        if (slot == nullptr) {
-          slot = my_epi + (epi_count & 1) * 2048;
-          if (epi_count >= 2) {
-            if (lane == 0) tma_store_wait_read<1>();
-            __syncwarp();
-          }
-        }
-        const long long gp_b = GP_NOW();
-        GP_ADD(4, gp_b - gp_a);
-        uint8_t* rowp = slot + lane * 64;
-        const int sw = (lane >> 1) & 3;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) *reinterpret_cast<uint4*>(rowp + ((j ^ sw) << 4)) = o[j];
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&p.tmC, slot, col, m_warp0);
-          tma_store_commit();
-        }
-        ++epi_count;
-        GP_ADD(5, GP_NOW() - gp_b);
-        GP_ADD(6, 1);
-      } else {
-        uint4* op = reinterpret_cast<uint4*>(p.out + m_row * p.ldo + col);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) op[j] = o[j];
-      }
-    };
-    // 16-column variant (GEGLU with 16 epilogue warps): 32-byte rows, no swizzle, tensor map tmC16 with box {16, 32}
-    auto store_chunk16 = [&](const uint4 (&o)[2], long long m_row, int col, int m_warp0) {
-      if (p.use_tma_store) {
-        uint8_t* slot = my_epi + (epi_count & 1) * kSlotBytes;
-        const long long gp_a = GP_NOW();
-        if (epi_count >= 2) {
-          if (lane == 0) tma_store_wait_read<1>();
-          __syncwarp();
-        }
-        const long long gp_b = GP_NOW();
-        GP_ADD(4, gp_b - gp_a);
-        *reinterpret_cast<uint4*>(slot + lane * 32) = o[0];
-        *reinterpret_cast<uint4*>(slot + lane * 32 + 16) = o[1];
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&p.tmC16, slot, col, m_warp0);
-          tma_store_commit();
-        }
-        ++epi_count;
-        GP_ADD(5, GP_NOW() - gp_b);
-        GP_ADD(6, 1);
-      } else {
-        uint4* op = reinterpret_cast<uint4*>(p.out + m_row * p.ldo + col);
-        op[0] = o[0];
-        op[1] = o[1];
-      }
-    };
-    // Coalesced residual fetch: lane l reads the 16-byte piece (l & 3) of rows (l >> 2) + 8 i of the warp's 32 x 32 block (8 lines
-    // per instruction instead of 32), the block is transposed through the staging slot and every lane picks up its own row.
-    const int r_piece = lane & 3, r_row0 = lane >> 2;
-    auto residual_fetch = [&](const __half* R, long long ld, int m_warp0, int col, uint4 (&pre)[4]) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const long long rr = static_cast<long long>(m_warp0) + r_row0 + 8 * i;
-        pre[i] = (rr < p.M) ? *reinterpret_cast<const uint4*>(R + rr * ld + col + r_piece * 8) : make_uint4(0, 0, 0, 0);
-      }
-    };
-    auto residual_add = [&](const uint4 (&pre)[4], uint8_t* slot, float (&v)[32]) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = r_row0 + 8 * i;
-        *reinterpret_cast<uint4*>(slot + r * 64 + ((r_piece ^ ((r >> 1) & 3)) << 4)) = pre[i];
-      }
-      __syncwarp();
-      const int sw = (lane >> 1) & 3;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint4 x = *reinterpret_cast<const uint4*>(slot + lane * 64 + ((j ^ sw) << 4));
-        const __half2* h = reinterpret_cast<const __half2*>(&x);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) { const float2 f = __half22float2(h[q]); v[8 * j + 2 * q] += f.x; v[8 * j + 2 * q + 1] += f.y; }
-      }
-      __syncwarp();
-    };
-    auto acquire_slot = [&]() -> uint8_t* {
-      if (epi_count >= 2) {
-        if (lane == 0) tma_store_wait_read<1>();
-        __syncwarp();
-      }
-      return my_epi + (epi_count & 1) * 2048;
-    };
-    int local = 0;
-    const long long gp_e0 = GP_NOW();
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-      const int buf = local & 1;
-      const uint32_t use = static_cast<uint32_t>(local >> 1);
-      const int mt = tile / p.n_tiles, nt = tile % p.n_tiles;
-      const long long m = static_cast<long long>(mt) * p.rows_per_tile + row_in_tile;
-      const bool row_ok = row_in_tile < p.rows_per_tile && m < p.M;
-      const long long gp_w = GP_NOW();
-      mbar_wait(&tfull[buf], use & 1);
-      GP_ADD(1, GP_NOW() - gp_w);
-      GP_ADD(7, 1);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + buf * BLOCK_N;
-      if (p.mode == FZ_EPI_GEGLU) {
-        constexpr int HALF = BLOCK_N / 2;
-        constexpr int CH = (HALF >= 32 && EPI_GROUPS == 2) ? 32 : 16;
-        if constexpr (HALF >= 16) {
-#pragma unroll 1
-          for (int c = half * CH; c < HALF; c += EPI_GROUPS * CH) {
-            uint32_t xa[CH], ga[CH];
-            const long long gp_l = GP_NOW();
-            if constexpr (CH == 32) {
-              tmem_ld_32x32b_x32(t_row + c, reinterpret_cast<uint32_t(&)[32]>(xa));
-              tmem_ld_32x32b_x32(t_row + HALF + c, reinterpret_cast<uint32_t(&)[32]>(ga));
-            } else {
-              tmem_ld_32x32b_x16(t_row + c, reinterpret_cast<uint32_t(&)[16]>(xa));
-              tmem_ld_32x32b_x16(t_row + HALF + c, reinterpret_cast<uint32_t(&)[16]>(ga));
-            }
-            tmem_ld_wait();
-            const long long gp_c = GP_NOW();
-            GP_ADD(2, gp_c - gp_l);
-            const int ocol0 = nt * HALF + c;
-            const int m_warp0 = mt * p.rows_per_tile + quad * 32;
-            const bool warp_ok = quad * 32 < p.rows_per_tile && m_warp0 < p.M;
-            if (warp_ok && ocol0 + CH <= p.N && (row_ok || (p.use_tma_store && (CH == 32 || EPI_GROUPS == 4)))) {
-              float xv[CH], gv[CH];
-#pragma unroll
-              for (int e = 0; e < CH; ++e) { xv[e] = __uint_as_float(xa[e]); gv[e] = __uint_as_float(ga[e]); }
-              // (prefetching these 64 bias values before the TMEM load was measured: the extra live registers spill under the
-              //  168-register cap of a 10-warp CTA and the epilogue gets 1.6x slower)
-              if (p.bias) {
-                const float4* bx = reinterpret_cast<const float4*>(p.bias + nt * BLOCK_N + c);
-                const float4* bg = reinterpret_cast<const float4*>(p.bias + nt * BLOCK_N + HALF + c);
-#pragma unroll
-                for (int j = 0; j < CH / 4; ++j) {
-                  const float4 a = __ldg(bx + j), b = __ldg(bg + j);
-                  xv[4 * j] += a.x; xv[4 * j + 1] += a.y; xv[4 * j + 2] += a.z; xv[4 * j + 3] += a.w;
-                  gv[4 * j] += b.x; gv[4 * j + 1] += b.y; gv[4 * j + 2] += b.z; gv[4 * j + 3] += b.w;
-                }
-              }
-              uint4 o[CH / 8];
-#pragma unroll
-              for (int j = 0; j < CH / 8; ++j) {
-                __half2 h0 = __floats2half2_rn(xv[8 * j + 0] * gelu_erf(gv[8 * j + 0]), xv[8 * j + 1] * gelu_erf(gv[8 * j + 1]));
-                __half2 h1 = __floats2half2_rn(xv[8 * j + 2] * gelu_erf(gv[8 * j + 2]), xv[8 * j + 3] * gelu_erf(gv[8 * j + 3]));
-                __half2 h2 = __floats2half2_rn(xv[8 * j + 4] * gelu_erf(gv[8 * j + 4]), xv[8 * j + 5] * gelu_erf(gv[8 * j + 5]));
-                __half2 h3 = __floats2half2_rn(xv[8 * j + 6] * gelu_erf(gv[8 * j + 6]), xv[8 * j + 7] * gelu_erf(gv[8 * j + 7]));
-                o[j].x = *reinterpret_cast<uint32_t*>(&h0); o[j].y = *reinterpret_cast<uint32_t*>(&h1);
-                o[j].z = *reinterpret_cast<uint32_t*>(&h2); o[j].w = *reinterpret_cast<uint32_t*>(&h3);
-              }
-              GP_ADD(3, GP_NOW() - gp_c);
-              if constexpr (CH == 32) {
-                store_chunk32(o, m, ocol0, m_warp0, nullptr);
-              } else if constexpr (EPI_GROUPS == 4) {
-                store_chunk16(o, m, ocol0, m_warp0);
-              } else {
-                uint4* op = reinterpret_cast<uint4*>(p.out + m * p.ldo + ocol0);
-#pragma unroll
-                for (int j = 0; j < CH / 8; ++j) op[j] = o[j];
-              }
-            } else if (row_ok) {
-#pragma unroll
-              for (int e = 0; e < CH; ++e) {
-                const int oc = ocol0 + e;
-                if (oc < p.N) {
-                  float xv = __uint_as_float(xa[e]), gv = __uint_as_float(ga[e]);
-                  if (p.bias) { xv += p.bias[nt * BLOCK_N + c + e]; gv += p.bias[nt * BLOCK_N + HALF + c + e]; }
-                  p.out[m * p.ldo + oc] = __float2half_rn(xv * gelu_erf(gv));
-                }
-              }
-            }
-          }
-        }
-      } else {
-        constexpr int CH = (BLOCK_N >= 32 && EPI_GROUPS == 2) ? 32 : 16;
-        const float* gb = p.group_bias ? p.group_bias + (m / p.rows_per_group) * p.N : nullptr;
-        uint4 preA[4], preB[4];
-        bool have_pre = false;
-#pragma unroll 1
-        for (int c = half * CH; c < BLOCK_N; c += EPI_GROUPS * CH) {
-          uint32_t acc[CH];
-          const long long gp_l = GP_NOW();
-          const int col0 = nt * BLOCK_N + c;
-          // the bias row of this chunk is fetched BEFORE the TMEM load so that its global-load latency overlaps it
-          float4 bvec[CH / 4];
-          const bool bias_pre = p.bias != nullptr && col0 + CH <= p.N;
-          if (bias_pre) {
-            const float4* bp = reinterpret_cast<const float4*>(p.bias + col0);
-#pragma unroll
-            for (int j = 0; j < CH / 4; ++j) bvec[j] = __ldg(bp + j);
-          }
-          if constexpr (CH == 32) tmem_ld_32x32b_x32(t_row + c, reinterpret_cast<uint32_t(&)[32]>(acc));
-          else tmem_ld_32x32b_x16(t_row + c, reinterpret_cast<uint32_t(&)[16]>(acc));
-          tmem_ld_wait();
-          const long long gp_c = GP_NOW();
-          GP_ADD(2, gp_c - gp_l);
-          const int m_warp0 = mt * p.rows_per_tile + quad * 32;
-          const bool warp_ok = quad * 32 < p.rows_per_tile && m_warp0 < p.M;
-          if (!warp_ok || col0 >= p.N) continue;
-          const bool fast = col0 + CH <= p.N && col0 + CH <= p.vt_col_start;
-          if (fast && (row_ok || (p.use_tma_store && (CH == 32 || EPI_GROUPS == 4)))) {
-            // ---------------- fast path: full chunk, row-major output ----------------
-            float v[CH];
-#pragma unroll
-            for (int e = 0; e < CH; ++e) v[e] = __uint_as_float(acc[e]);
-            if (bias_pre) {
-#pragma unroll
-              for (int j = 0; j < CH / 4; ++j) {
-                const float4 b = bvec[j];
-                v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-              }
-            }
-            if (gb && row_ok) {
-              const float4* bp = reinterpret_cast<const float4*>(gb + col0);
-#pragma unroll
-              for (int j = 0; j < CH / 4; ++j) {
-                const float4 b = __ldg(bp + j);
-                v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-              }
-            }
-            uint8_t* slot = nullptr;
-            if constexpr (CH == 32) {
-              if (p.use_tma_store && (p.residual || p.residual2)) {
-                slot = acquire_slot();
-                if (!have_pre) {
-                  if (p.residual) residual_fetch(p.residual, p.ldr, m_warp0, col0, preA);
-                  if (p.residual2) residual_fetch(p.residual2, p.ldr2, m_warp0, col0, preB);
-                }
-                if (p.residual) residual_add(preA, slot, v);
-                if (p.residual2) residual_add(preB, slot, v);
-                // software pipeline: issue the next chunk's residual loads now, consume them after its TMEM load
-                const int c_next = c + 2 * CH;
-                const int col_next = nt * BLOCK_N + c_next;
-                have_pre = c_next < BLOCK_N && col_next + CH <= p.N && col_next + CH <= p.vt_col_start;
-                if (have_pre) {
-                  if (p.residual) residual_fetch(p.residual, p.ldr, m_warp0, col_next, preA);
-                  if (p.residual2) residual_fetch(p.residual2, p.ldr2, m_warp0, col_next, preB);
-                }
-              }
-            }
-            if (slot == nullptr) {
-              if (p.residual && row_ok) {
-                const uint4* rp = reinterpret_cast<const uint4*>(p.residual + m * p.ldr + col0);
-#pragma unroll
-                for (int j = 0; j < CH / 8; ++j) {
-                  const uint4 r = rp[j];
-                  const __half2* h = reinterpret_cast<const __half2*>(&r);
-#pragma unroll
-                  for (int q = 0; q < 4; ++q) { const float2 f = __half22float2(h[q]); v[8 * j + 2 * q] += f.x; v[8 * j + 2 * q + 1] += f.y; }
-                }
-              }
-              if (p.residual2 && row_ok) {
-                const uint4* rp = reinterpret_cast<const uint4*>(p.residual2 + m * p.ldr2 + col0);
-#pragma unroll
-                for (int j = 0; j < CH / 8; ++j) {
-                  const uint4 r = rp[j];
-                  const __half2* h = reinterpret_cast<const __half2*>(&r);
-#pragma unroll
-                  for (int q = 0; q < 4; ++q) { const float2 f = __half22float2(h[q]); v[8 * j + 2 * q] += f.x; v[8 * j + 2 * q + 1] += f.y; }
-                }
-              }
-            }
-            uint4 o[CH / 8];
-#pragma unroll
-            for (int j = 0; j < CH / 8; ++j) {
-              __half2 h0 = __floats2half2_rn(v[8 * j + 0], v[8 * j + 1]), h1 = __floats2half2_rn(v[8 * j + 2], v[8 * j + 3]);
-              __half2 h2 = __floats2half2_rn(v[8 * j + 4], v[8 * j + 5]), h3 = __floats2half2_rn(v[8 * j + 6], v[8 * j + 7]);
-              o[j].x = *reinterpret_cast<uint32_t*>(&h0); o[j].y = *reinterpret_cast<uint32_t*>(&h1);
-              o[j].z = *reinterpret_cast<uint32_t*>(&h2); o[j].w = *reinterpret_cast<uint32_t*>(&h3);
-            }
-            GP_ADD(3, GP_NOW() - gp_c);
-            if constexpr (CH == 32) {
-              store_chunk32(o, m, col0, m_warp0, slot);
-            } else if constexpr (EPI_GROUPS == 4) {
-              store_chunk16(o, m, col0, m_warp0);
-            } else {
-              uint4* op = reinterpret_cast<uint4*>(p.out + m * p.ldo + col0);
-#pragma unroll
-              for (int j = 0; j < CH / 8; ++j) op[j] = o[j];
-            }
-          } else if (CH == 32 && p.vt_tma && col0 >= p.vt_col_start && col0 + CH <= p.N) {
-            // ---------------- V^T store, staged: the warp's 32 tokens x 32 columns are transposed through its staging slot ([column][token],
-            // 64-byte rows) and leave as ONE bulk tensor store into out_vt viewed as [BF * heads * d, S] (the per-element variant below
-            // issued 32 two-byte global stores per thread: 65536 x 960 x 320 ran 90 us against 30 us for a row-major GEMM of 1/3 the columns)
-            if constexpr (CH == 32) {
-              uint8_t* slot = acquire_slot();
-              // 2 x 2 transposes between neighbouring lanes: an even lane keeps column 2j of tokens (lane, lane + 1), the odd lane column 2j + 1
-              // of tokens (lane - 1, lane): 16 shuffles + 16 conflict-free 4-byte st.shared per thread instead of 32 two-byte stores
-              const bool odd = lane & 1;
-              uint32_t* wp = reinterpret_cast<uint32_t*>(slot) + (lane >> 1);
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                float v0 = __uint_as_float(acc[2 * j]), v1 = __uint_as_float(acc[2 * j + 1]);
-                if (p.bias) { v0 += __ldg(p.bias + col0 + 2 * j); v1 += __ldg(p.bias + col0 + 2 * j + 1); }
-                const float got = __shfl_xor_sync(0xffffffffu, odd ? v0 : v1, 1);
-                wp[(2 * j + (odd ? 1 : 0)) * 16] = odd ? pack_h2(got, v1) : pack_h2(v0, got);
-              }
-              fence_proxy_async_smem();
-              __syncwarp();
-              if (lane == 0) {
-                const int bfi = m_warp0 / p.vt_S;
-                tma_store_2d(&p.tmVt, slot, m_warp0 - bfi * p.vt_S, bfi * (p.N - p.vt_col_start) + (col0 - p.vt_col_start));
-                tma_store_commit();
-              }
-              ++epi_count;
-            }
-          } else if (col0 >= p.vt_col_start) {
-            // ---------------- V^T store: out_vt[((bf*heads + h)*d + dd)*ld + s]; lanes = consecutive s -> 64-byte segments ----------------
-            if (!row_ok) continue;
-            const long long bf = m / p.vt_S;
-            const int s = static_cast<int>(m % p.vt_S);
-            const int cv0 = col0 - p.vt_col_start;
-            int h = cv0 / p.vt_d, dd = cv0 % p.vt_d;
-            __half* vbase = p.out_vt + (bf * p.vt_heads) * static_cast<long long>(p.vt_d) * p.vt_ld + s;
-#pragma unroll
-            for (int e = 0; e < CH; ++e) {
-              if (col0 + e < p.N) {
-                float v = __uint_as_float(acc[e]);
-                if (p.bias) v += p.bias[col0 + e];
-                vbase[(static_cast<long long>(h) * p.vt_d + dd) * p.vt_ld] = __float2half_rn(v);
-              }
-              if (++dd == p.vt_d) { dd = 0; ++h; }
-            }
-          } else {
-            // ---------------- generic masked path (right-edge tiles, chunks straddling vt_col_start) ----------------
-            if (!row_ok) continue;
-#pragma unroll
-            for (int e = 0; e < CH; ++e) {
-              const int col = col0 + e;
-              if (col >= p.N) continue;
-              float v = __uint_as_float(acc[e]);
-              if (p.bias) v += p.bias[col];
-              if (col >= p.vt_col_start) {
-                const long long bf = m / p.vt_S;
-                const int s = static_cast<int>(m % p.vt_S);
-                const int cv = col - p.vt_col_start;
-                p.out_vt[((bf * p.vt_heads + cv / p.vt_d) * p.vt_d + cv % p.vt_d) * p.vt_ld + s] = __float2half_rn(v);
-              } else {
-                if (gb) v += gb[col];
-                if (p.residual) v += __half2float(p.residual[m * p.ldr + col]);
-                if (p.residual2) v += __half2float(p.residual2[m * p.ldr2 + col]);
-                p.out[m * p.ldo + col] = __float2half_rn(v);
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[buf]);
-    }
-    // the staging slots must stay valid until the bulk stores have READ them; their global writes complete with the grid
-    // (kernel boundary / griddepcontrol.wait of the dependent), as in CUTLASS' store_tail
-    if ((p.use_tma_store || p.vt_tma) && lane == 0) tma_store_wait_read<0>();
-#ifdef FZ_GEMM_PROFILE
-    if (gp_on && warp == 2 && lane == 0) {
-      g_gemm_dbg[0] = GP_NOW() - gp_e0;
-      for (int i = 1; i < 8; ++i) g_gemm_dbg[i] = gp[i];
-    }
-#endif
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+
+  // ===================== consumer warpgroups: wgmma mainloop + epilogue =====================
+  const int lane = threadIdx.x & 31;
+  const int warp_in = (threadIdx.x >> 5) & 3;
+  const uint64_t desc0 = wgmma_desc_k_sw128(smem_u32(smem));
+  float acc[BLOCK_N / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  // accumulator fragment: acc[4 i + 2 h + j] = tile row r_base + 8 h, tile column 8 i + c_base + j
+  const int r_base = wg * 64 + warp_in * 16 + (lane >> 2);
+  const int c_base = 2 * (lane & 3);
+  const bool pair_ok = (p.ldo % 2) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 3) == 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int mt = tile / p.n_tiles, nt = tile % p.n_tiles;
+    int prev = -1;
+    for (int it = 0; it < k_iters; ++it) {
+      mbar_wait(&full[stage], phase);
+      const uint64_t da = desc0 + static_cast<uint32_t>((stage * Cfg::kStageBytes + wg * 64 * 128) >> 4);
+      const uint64_t db = desc0 + static_cast<uint32_t>((stage * Cfg::kStageBytes + kATileBytes) >> 4);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k) wgmma_f16<BLOCK_N>(acc, da + 2 * k, db + 2 * k, (it | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous stage's MMAs are done: hand its buffers back to the producer
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r_base + 8 * h;
+      const long long m = static_cast<long long>(mt) * p.rows_per_tile + r;
+      if (r >= p.rows_per_tile || m >= p.M) continue;
+      if (p.mode == FZ_EPI_GEGLU) {
+        // x columns [0, HALF) and gate columns [HALF, BLOCK_N) of the tile sit in the same thread (HALF is a multiple of 8)
+        constexpr int HALF = BLOCK_N / 2;
+        if constexpr (HALF % 8 == 0) {
+          __half* orow = p.out + m * p.ldo;
+#pragma unroll
+          for (int i = 0; i < HALF / 8; ++i) {
+            const int c = 8 * i + c_base;
+            const int oc = nt * HALF + c;
+            if (oc >= p.N) continue;
+            float x0 = acc[4 * i + 2 * h], x1 = acc[4 * i + 2 * h + 1];
+            float g0 = acc[4 * (i + HALF / 8) + 2 * h], g1 = acc[4 * (i + HALF / 8) + 2 * h + 1];
+            if (p.bias) {
+              const float* b = p.bias + nt * BLOCK_N + c;
+              x0 += __ldg(b); x1 += __ldg(b + 1); g0 += __ldg(b + HALF); g1 += __ldg(b + HALF + 1);
+            }
+            const float o0 = x0 * gelu_erf(g0), o1 = x1 * gelu_erf(g1);
+            if (pair_ok && oc + 1 < p.N) {
+              *reinterpret_cast<__half2*>(orow + oc) = __floats2half2_rn(o0, o1);
+            } else {
+              orow[oc] = __float2half_rn(o0);
+              if (oc + 1 < p.N) orow[oc + 1] = __float2half_rn(o1);
+            }
+          }
+        }
+      } else {
+        const float* gb = p.group_bias ? p.group_bias + (m / p.rows_per_group) * p.N : nullptr;
+        __half* orow = p.out + m * p.ldo;
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 8; ++i) {
+          const int col = nt * BLOCK_N + 8 * i + c_base;
+          if (col >= p.N) continue;
+          float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+          if (pair_ok && col + 2 <= p.N && col + 2 <= p.vt_col_start) {
+            if (p.bias) { v0 += __ldg(p.bias + col); v1 += __ldg(p.bias + col + 1); }
+            if (gb) { v0 += __ldg(gb + col); v1 += __ldg(gb + col + 1); }
+            if (p.residual) { v0 += __half2float(p.residual[m * p.ldr + col]); v1 += __half2float(p.residual[m * p.ldr + col + 1]); }
+            if (p.residual2) { v0 += __half2float(p.residual2[m * p.ldr2 + col]); v1 += __half2float(p.residual2[m * p.ldr2 + col + 1]); }
+            *reinterpret_cast<__half2*>(orow + col) = __floats2half2_rn(v0, v1);
+          } else {
+            epi_store1(p, m, col, v0, gb);
+            if (col + 1 < p.N) epi_store1(p, m, col + 1, v1, gb);
+          }
+        }
+      }
+    }
   }
 }
 
@@ -650,35 +274,24 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
 }
 
-template <int BN, int EG>
-static int launch_tapgemm_eg(const TapGemmParams& p, cudaStream_t stream) {
+template <int BN>
+static int launch_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
   using Cfg = TapGemmCfg<BN>;
   static bool configured = false;
   if (!configured) {
-    FZ_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN, EG>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    FZ_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     configured = true;
   }
   const int tiles = p.m_tiles * p.n_tiles;
   const int grid = std::min(tiles, num_sms());
-  FZ_CUDA(launch_pdl(tapgemm_kernel<BN, EG>, dim3(grid), dim3(64 + 128 * EG), Cfg::kSmemBytes, stream, p));
+  FZ_CUDA(launch_pdl(tapgemm_kernel<BN>, dim3(grid), dim3(384), Cfg::kSmemBytes, stream, p));
   FZ_CUDA(cudaGetLastError());
   return FZ_OK;
-}
-
-template <int BN>
-static int launch_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
-  if constexpr (BN >= 64) {
-    // 16 epilogue warps (16-column chunks, 96 registers) for the ALU-bound GEGLU epilogue.  Measured and rejected for the short-K
-    // row-major GEMMs: their chunks are latency-bound (~860 cycles per chunk whether it is 16 or 32 columns wide), so twice the warps on
-    // half-size chunks gain nothing (65536x320x320: epilogue warp 29.1k -> 39.5k cycles).
-    if (p.use_tma_store == 2 && p.mode == FZ_EPI_GEGLU) return launch_tapgemm_eg<BN, 4>(p, stream);
-  }
-  return launch_tapgemm_eg<BN, 2>(p, stream);
 }
 
 static int pick_block_n(int gemm_cols, int mode, int forced, int m_tiles) {
@@ -760,30 +373,6 @@ static int fold_residuals(TapGemmParams& p, int bn, cudaStream_t stream) {
 
 static int dispatch_tapgemm(TapGemmParams& p, int gemm_cols, int forced_bn, cudaStream_t stream) {
   if (int rc = check_single_device()) return rc;
-  // output tensor map for the TMA-store epilogue ([M, N_out] row-major, row stride ldo)
-  p.use_tma_store = 0;
-  if (p.rows_per_tile % 32 == 0 && p.ldo % 8 == 0 && p.N % 8 == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 &&
-      std::min(p.N, p.vt_col_start) >= 32) {
-    uint64_t dims[2] = {static_cast<uint64_t>(std::min(p.N, p.vt_col_start)), static_cast<uint64_t>(p.M)};
-    uint64_t strides[1] = {static_cast<uint64_t>(p.ldo)};
-    uint32_t box[2] = {32, 32};
-    if (int rc = encode_tmap_f16_sw(&p.tmC, p.out, 2, dims, strides, box, 64)) return rc;
-    p.use_tma_store = 1;
-    if (p.N % 16 == 0 && (p.vt_col_start == INT_MAX || p.vt_col_start % 16 == 0)) {
-      uint32_t box16[2] = {16, 32};
-      if (int rc = encode_tmap_f16_sw(&p.tmC16, p.out, 2, dims, strides, box16, 0)) return rc;
-      p.use_tma_store = 2;  // both maps valid: the GEGLU launch may take the 16-epilogue-warp instantiation
-    }
-  }
-  p.vt_tma = 0;
-  if (p.out_vt && p.vt_S % 32 == 0 && p.rows_per_tile % 32 == 0 && p.vt_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(p.out_vt) & 15) == 0 &&
-      p.vt_col_start % 32 == 0 && p.N - p.vt_col_start == p.vt_heads * p.vt_d && p.M % p.vt_S == 0) {
-    uint64_t dims[2] = {static_cast<uint64_t>(p.vt_S), static_cast<uint64_t>(p.M / p.vt_S) * (p.N - p.vt_col_start)};
-    uint64_t strides[1] = {static_cast<uint64_t>(p.vt_ld)};
-    uint32_t box[2] = {32, 32};
-    if (int rc = encode_tmap_f16_sw(&p.tmVt, p.out_vt, 2, dims, strides, box, 0)) return rc;
-    p.vt_tma = 1;
-  }
   const int bn = pick_block_n(gemm_cols, p.mode, forced_bn, p.m_tiles);
   p.n_tiles = (gemm_cols + bn - 1) / bn;
   if (int rc = fold_residuals(p, bn, stream)) return rc;
@@ -822,14 +411,6 @@ static int fill_epilogue(TapGemmParams& p, const fz_epilogue_t* e, int M, int ge
 }  // namespace fz
 
 using namespace fz;
-
-// Development aid (not part of include/fatezero_b200.h): cycle counters of the last tap-GEMM launch, zeros unless built with
-// -DFZ_GEMM_PROFILE (tools/profile_gemm_epilogue.py).
-extern "C" int fz_debug_gemm_counters(long long* host16) {
-  FZ_CUDA(cudaDeviceSynchronize());
-  FZ_CUDA(cudaMemcpyFromSymbol(host16, g_gemm_dbg, sizeof(long long) * 16));
-  return FZ_OK;
-}
 
 // One-time device-side initialisation (constant tables).  Idempotent; must have run before the first call under stream capture.
 extern "C" int fz_init(cudaStream_t stream) {

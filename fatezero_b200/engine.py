@@ -1,4 +1,4 @@
-"""UNetEngine — executes one UNetPseudo3DConditionModel forward with the sm_100a kernels of libfatezero_b200.so.
+"""UNetEngine — executes one UNetPseudo3DConditionModel forward with the sm_90a kernels of libfatezero_b200.so.
 
 Data layout in HBM: every activation is fp16 channels-last, `[B*F, H, W, C]` == token-major `[B*F*H*W, C]` (frame-minor batch
 order like the reference's "(b f)" rearranges), so conv / linear / attention kernels read and write the same buffers without
@@ -49,7 +49,7 @@ class UNetEngine:
     def __init__(self, unet, exact_skips: bool = True):
         dev = unet.device
         if dev.type != "cuda":
-            raise RuntimeError("UNetEngine needs the UNet parameters on a CUDA device (sm_100a); no CPU fallback exists")
+            raise RuntimeError("UNetEngine needs the UNet parameters on a CUDA device (sm_90a); no CPU fallback exists")
         lib = _lib.load()
         _lib.check(lib.fz_device_check(), "fz_device_check")
         with torch.cuda.device(dev):

@@ -38,6 +38,10 @@ class StepGraphs:
 
     def capture(self, fn: Callable[[], None]):
         """Capture fn() (which must only enqueue work on the current stream) as the next step graph."""
+        if not self.graphs:
+            # The private pool cannot reuse blocks cached by the ordinary pool, e.g. a previous clip's freed map cache (36 GiB at
+            # 512x512x8f): hand them back to the device so that the captured loop fits next to them on an 80 GB card.
+            torch.cuda.empty_cache()
         g = torch.cuda.CUDAGraph()
         cur = torch.cuda.current_stream(self.device)
         self.stream.wait_stream(cur)

@@ -97,7 +97,7 @@ class SpatioTemporalStableDiffusionPipeline:
         self._progress_bar_config = kwargs
 
     def enable_xformers_memory_efficient_attention(self, *a, **k):
-        return None  # the fused sm_100a attention kernel is always on
+        return None  # the fused sm_90a attention kernel is always on
 
     def disable_xformers_memory_efficient_attention(self, *a, **k):
         return None
@@ -141,7 +141,7 @@ class SpatioTemporalStableDiffusionPipeline:
 
     def _text_forward(self, ids, mask):
         """The text encoder call of stable_diffusion.py:230,279.  A transformers CLIPTextModel living on the GPU is executed by
-        clip.ClipTextEngine (sm_100a kernels, built once per module); any other module — or a padding mask — is simply called."""
+        clip.ClipTextEngine (sm_90a kernels, built once per module); any other module — or a padding mask — is simply called."""
         te = self.text_encoder
         if (mask is None and os.environ.get("FZ_CLIP", "1") != "0" and type(te).__name__ == "CLIPTextModel" and isinstance(te, torch.nn.Module)
                 and next(te.parameters()).is_cuda):
@@ -188,7 +188,7 @@ class SpatioTemporalStableDiffusionPipeline:
         return emb
 
     def _vae_engine(self):
-        """The sm_100a VAE executor for `self.vae` (fatezero_b200.vae): our AutoencoderKL container or a foreign AutoencoderKL-shaped
+        """The sm_90a VAE executor for `self.vae` (fatezero_b200.vae): our AutoencoderKL container or a foreign AutoencoderKL-shaped
         module on the GPU; None for anything else (stubs, CPU modules) — those are simply called."""
         if os.environ.get("FZ_VAE", "1") == "0":
             return None

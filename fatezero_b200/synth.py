@@ -2,7 +2,7 @@
 
 There is no network and no SD checkpoint on the build or GPU boxes (SURVEY.md §8(c)/(d)), so every test and bench
 run uses random weights of the right geometry.  The recipe below is *name-keyed* (one RNG stream per state-dict key),
-so the reference UNet (built through the oracle shim), the CPU oracle and the B200 engine all get bit-identical
+so the reference UNet (built through the oracle shim), the CPU oracle and the CUDA engine all get bit-identical
 weights without depending on module construction order.
 """
 from __future__ import annotations

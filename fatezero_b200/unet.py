@@ -4,7 +4,7 @@
 The module owns fp32 parameters under EXACTLY the reference's state-dict names / shapes (SURVEY.md App. E3), so
 `from_2d_model` / `load_2d_state_dict` / `load_state_dict` accept Stable-Diffusion-1.x and Tune-A-Video checkpoints
 unchanged.  `forward` does not run PyTorch layers: it hands the tensors to `engine.UNetEngine`, which executes the
-step with the sm_100a kernels of libfatezero_b200.so (there is no CPU / eager fallback).
+step with the sm_90a kernels of libfatezero_b200.so (there is no CPU / eager fallback).
 """
 from __future__ import annotations
 
@@ -265,7 +265,7 @@ class UNetPseudo3DConditionModel(nn.Module):
         if class_labels is not None or attention_mask is not None:
             raise NotImplementedError("class_labels / attention_mask are not supported (attention_register.py:146-151)")
         if not sample.is_cuda:
-            raise RuntimeError("fatezero_b200.UNetPseudo3DConditionModel runs on CUDA (sm_100a) only; move the model and inputs to "
+            raise RuntimeError("fatezero_b200.UNetPseudo3DConditionModel runs on CUDA (sm_90a) only; move the model and inputs to "
                                "the GPU — there is no CPU fallback")
         t = float(timestep.item()) if torch.is_tensor(timestep) else float(timestep)
         if sample.device != self.device:

@@ -1,4 +1,4 @@
-"""VAE encode / decode on the sm_100a kernels (SURVEY.md §8(f) rank 1): the `AutoencoderKL` the reference brackets its hot path with
+"""VAE encode / decode on the sm_90a kernels (SURVEY.md §8(f) rank 1): the `AutoencoderKL` the reference brackets its hot path with
 (`pipelines/p2p_ddim_spatial_temporal.py:88-96`: `vae.encode(image).latent_dist.sample(generator)`; `pipelines/stable_diffusion.py:297-319`:
 `vae.decode(latents).sample` in chunks of 16 frames).
 
@@ -8,7 +8,7 @@ AttentionBlock / UpDecoderBlock2D, GroupNorm(32, eps 1e-6) + SiLU, no time embed
     downsample is the right/bottom-padded stride-2 variant `fz_conv3x3_down_asym_nhwc_f16`), 1x1 shortcuts and attention projections are
     `fz_gemm_f16`, the RGB / latent input convs go through the im2col GEMM like the UNet's conv_in;
   * GroupNorm(+SiLU), nearest upsampling: the UNet's HBM-bound kernels;
-  * the mid-block attention (one head of width 512: more than the fused attention kernels hold in TMEM) runs per image as
+  * the mid-block attention (one head of width 512: more than the fused attention kernel holds in registers) runs per image as
     GEMM (Q K^T) -> `fz_softmax_rows_f16` -> GEMM (P V^T with V^T produced directly by a GEMM with swapped operands; the value bias is
     added after P V, exact because the probabilities of a row sum to one).
 fp16 storage / fp32 accumulation, fp32 in and out.  `AutoencoderKL` below is a parameter container with the diffusers state-dict names and
@@ -117,7 +117,7 @@ class _Out(dict):
 class VaeEngine:
     def __init__(self, state_dict: Dict[str, torch.Tensor], cfg: dict, device: torch.device):
         if torch.device(device).type != "cuda":
-            raise RuntimeError("VaeEngine needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("VaeEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.dev = torch.device(device)
         self.cfg = dict(cfg)
         self.ch = list(cfg["block_out_channels"])

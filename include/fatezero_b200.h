@@ -1,4 +1,4 @@
-/* fatezero_b200.h — C ABI of libfatezero_b200.so (sm_100a kernels of the FateZero hot path).
+/* fatezero_b200.h — C ABI of libfatezero_b200.so (sm_90a kernels of the FateZero hot path).
  *
  * The reference (ChenyangQiQi/FateZero) has NO native boundary: its seam is Python duck-typing
  * (SURVEY.md §8(b)).  This header therefore defines the boundary the drop-in Python package
@@ -23,14 +23,14 @@ typedef struct CUstream_st* fz_stream_t; /* == cudaStream_t */
 
 const char* fz_last_error(void);
 int fz_version(void);
-/* Runtime probe: returns 0 when the current device is sm_100 and the kernels can run. */
+/* Runtime probe: returns 0 when the current device is sm_90 and the kernels can run. */
 int fz_device_check(void);
 /* One-time device-side initialisation (constant tables; synchronises `stream` the first time).  Idempotent.  Must have run before the
  * library is first used under CUDA-graph stream capture (fatezero_b200.engine.UNetEngine calls it at construction). */
 int fz_init(fz_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Tap-GEMM family (tcgen05 / TMEM / TMA).  D[M,N] = sum_tap A_tap[M,K] W_tap[N,K]^T  (+ fused epilogue)
+ * Tap-GEMM family (wgmma / TMA).  D[M,N] = sum_tap A_tap[M,K] W_tap[N,K]^T  (+ fused epilogue)
  * --------------------------------------------------------------------------------------------------------- */
 enum { FZ_EPI_ROWMAJOR = 0, FZ_EPI_GEGLU = 1 };
 
@@ -105,7 +105,7 @@ typedef struct fz_attn_args {
   void* acc;       long long acc_ld;/* fp16 running sum slab or NULL (attention_store.py:95-101)                    */
   const float* xedit;               /* device table, see above                                                       */
   const float* mask;                /* device [BF-edit_bf_start, S_q], 1 = keep current row                          */
-  void* dbg;                        /* optional device int64[32]: cycle counters of CTA (0,0,0) (profiling aid) or NULL */
+  void* dbg;                        /* reserved, ignored (may be NULL)                                                   */
   int causal;                       /* 1: key n is visible to query s only if n <= s (CLIP text encoder; needs n_slots == 1, row_mode NONE) */
 } fz_attn_args_t;
 

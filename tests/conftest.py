@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -19,7 +19,7 @@ def pytest_collection_modifyitems(config, items):
     lib = os.path.join(ROOT, "fatezero_b200", "libfatezero_b200.so")
     reason = None
     if not torch.cuda.is_available():
-        reason = "needs a CUDA device (B200)"
+        reason = "needs a CUDA device (H100)"
     elif not os.path.exists(lib):
         reason = f"{lib} is not built (python -c 'import __graft_entry__ as g; g.build()')"
     if reason is None:

@@ -1,10 +1,10 @@
 """Drop-in boundary (SURVEY.md §8(b)): the reference's UNCHANGED `P2pSampleLogger.log_sample_images`
 (video_diffusion/pipelines/p2p_validation_loop.py:68-131) must be able to drive this repo's pipeline.
 
-Two halves, because the reference tree only exists in the build container and the GPU only on the GPU box:
-  * CPU, reference present: import the reference's logger THROUGH this repo's `video_diffusion` alias package (modules the alias does not
-    provide fall through to the reference tree), run `log_sample_images` against a recording pipeline, and bind every recorded call to
-    the signature of our `P2pDDIMSpatioTemporalPipeline.__call__` / `sd_ddim_pipeline` / `make_controller`;
+Two halves:
+  * CPU: the keyword arguments of every pipeline call the reference's logger makes (recorded once by running `log_sample_images`, imported
+    through this repo's `video_diffusion` alias package, against a recording pipeline: tests/golden/ref_logger_calls.json) are bound to the
+    signature of our `P2pDDIMSpatioTemporalPipeline.sd_ddim_pipeline` / `make_controller`;
   * GPU: the same call sequence (kwargs as recorded there, cited line by line) against the real CUDA pipeline with stub VAE / tokenizer."""
 import inspect
 import os
@@ -17,7 +17,6 @@ import torch
 from _helpers import ROOT, build_product
 from fatezero_b200 import synth
 
-REF = "/root/reference"
 SRC = "a silver jeep driving down a curvy road in the countryside"
 EDITS = [SRC, "watercolor painting of " + SRC]
 P2P = {0: dict(is_replace_controller=False, cross_replace_steps={"default_": 0.8}, self_replace_steps=0.9, blend_self_attention=True),
@@ -34,55 +33,24 @@ def logger_kwargs(idx, prompt, image, latents, save_dir, steps, clip_length):
                 uncond_embeddings_list=None, save_path=save_dir, **cfg)
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "video_diffusion")), reason="reference tree only exists in the build container")
-def test_unchanged_reference_logger_binds_to_our_pipeline(tmp_path):
-    code = r'''
-import inspect, json, sys, types
-import numpy as np, torch
-from PIL import Image
-sys.path.insert(0, %(root)r); sys.path.insert(0, %(root)r + "/oracle/shim"); sys.path.append(%(ref)r)
-import video_diffusion                                        # THIS repo's alias package ...
-from video_diffusion.pipelines.p2p_validation_loop import P2pSampleLogger   # ... falling through to the reference's own file
-import video_diffusion.pipelines.p2p_validation_loop as m
-assert m.__file__.startswith(%(ref)r), m.__file__
-from video_diffusion.pipelines.p2p_ddim_spatial_temporal import P2pDDIMSpatioTemporalPipeline as Ours
-assert Ours.__module__ == "fatezero_b200.pipeline", Ours.__module__
-from fatezero_b200 import controllers
-
-calls = []
-class Recorder:
-    @staticmethod
-    def numpy_to_pil(x):
-        return Ours.numpy_to_pil(x)
-    def __call__(self, **kw):
-        calls.append(kw)
-        frames = [Image.fromarray(np.zeros((16, 16, 3), np.uint8)) for _ in range(2)]
-        return {"sdimage_output": types.SimpleNamespace(images=[frames]), "attention_output": None, "mask_list": None}
-
-p2p = %(p2p)r
-lg = P2pSampleLogger(editing_prompts=%(edits)r, clip_length=2, logdir=%(tmp)r, num_inference_steps=3, guidance_scale=7.5, sample_seeds=[0],
-                     prompt2prompt_edit=True, p2p_config=p2p, use_inversion_attention=True, source_prompt=%(src)r)
-lg.log_sample_images(pipeline=Recorder(), device=torch.device("cpu"), step=0, image=torch.zeros(2, 3, 16, 16), latents=torch.zeros(1, 4, 2, 4, 4),
-                     save_dir=%(tmp)r)
-assert len(calls) == 2
-sig_call = inspect.signature(Ours.sd_ddim_pipeline)
-mk = inspect.signature(controllers.make_controller)
-for kw in calls:
-    assert kw["edit_type"] == "swap" and kw["use_inversion_attention"] is True and kw["save_self_attention"] is False
-    bound = sig_call.bind(None, controller=None, **kw)     # **args swallows what sd_ddim_pipeline does not name (p2p_ddim_spatial_temporal.py:280)
-    # p2preplace_edit (p2p_ddim_spatial_temporal.py:172-222) forwards these keys to make_controller under these names
-    mk.bind(None, [kw["source_prompt"], kw["prompt"]], NUM_DDIM_STEPS=kw["num_inference_steps"], is_replace_controller=kw.get("is_replace_controller", True),
-            cross_replace_steps=kw["cross_replace_steps"], self_replace_steps=kw["self_replace_steps"], blend_words=kw.get("blend_words"),
-            equilizer_params=kw.get("eq_params"), additional_attention_store=None, use_inversion_attention=kw["use_inversion_attention"],
-            blend_th=kw.get("blend_th", (0.3, 0.3)), blend_self_attention=kw.get("blend_self_attention"), blend_latents=kw.get("blend_latents"),
-            save_path=kw.get("save_path"), save_self_attention=kw.get("save_self_attention", True), disk_store=kw.get("disk_store", False))
-print(json.dumps(sorted(calls[1].keys())))
-''' % dict(root=ROOT, ref=REF, p2p=P2P, edits=EDITS, tmp=str(tmp_path / "log"), src=SRC)
-    import subprocess
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stdout[-1500:] + r.stderr[-3000:]
+def test_unchanged_reference_logger_binds_to_our_pipeline():
     import json
-    recorded = set(json.loads(r.stdout.strip().splitlines()[-1]))
+    from fatezero_b200 import controllers
+    from fatezero_b200.pipeline import P2pDDIMSpatioTemporalPipeline as Ours
+    calls = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_logger_calls.json")))
+    assert len(calls) == 2
+    sig_call = inspect.signature(Ours.sd_ddim_pipeline)
+    mk = inspect.signature(controllers.make_controller)
+    for kw in calls:
+        assert kw["edit_type"] == "swap" and kw["use_inversion_attention"] is True and kw["save_self_attention"] is False
+        sig_call.bind(None, controller=None, **kw)  # **args swallows what sd_ddim_pipeline does not name (p2p_ddim_spatial_temporal.py:280)
+        # p2preplace_edit (p2p_ddim_spatial_temporal.py:172-222) forwards these keys to make_controller under these names
+        mk.bind(None, [kw["source_prompt"], kw["prompt"]], NUM_DDIM_STEPS=kw["num_inference_steps"], is_replace_controller=kw.get("is_replace_controller", True),
+                cross_replace_steps=kw["cross_replace_steps"], self_replace_steps=kw["self_replace_steps"], blend_words=kw.get("blend_words"),
+                equilizer_params=kw.get("eq_params"), additional_attention_store=None, use_inversion_attention=kw["use_inversion_attention"],
+                blend_th=kw.get("blend_th", (0.3, 0.3)), blend_self_attention=kw.get("blend_self_attention"), blend_latents=kw.get("blend_latents"),
+                save_path=kw.get("save_path"), save_self_attention=kw.get("save_self_attention", True), disk_store=kw.get("disk_store", False))
+    recorded = set(calls[1])
     mine = set(logger_kwargs(1, EDITS[1], None, None, None, 3, 2).keys())
     assert recorded == mine, (recorded ^ mine)   # the GPU half below replays exactly the keyword set the reference logger sends
 

@@ -1,5 +1,7 @@
 """CPU-side checks: the C-ABI library loads and exports every declared symbol, the parameter spec equals the reference's state dict,
 the reference-facing surface exists and refuses to run without CUDA, and the N>1 plumbing works under gloo (world_size 2)."""
+import gzip
+import json
 import os
 import re
 import subprocess
@@ -9,6 +11,8 @@ import pytest
 import torch
 
 from _helpers import ROOT
+from fatezero_b200 import synth
+from fatezero_b200.unet import unet_param_spec
 
 
 def test_library_exports_every_header_symbol():
@@ -45,30 +49,21 @@ def test_spec_counts():
     assert abs(n2 - 1060e6) < 2e6
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference tree only exists in the build container")
 def test_spec_equals_reference_state_dict():
-    code = r'''
-import sys
-sys.path.insert(0, %r)
-from oracle import ref_harness as rh
-rh._prepare_imports()
-from video_diffusion.models.unet_3d_condition import UNetPseudo3DConditionModel as Ref
-from fatezero_b200 import synth
-from fatezero_b200.unet import unet_param_spec
-for mc in (dict(lora=160, SparseCausalAttention_index=["mid"], least_sc_channel=128), dict(), dict(lora=8)):
-    ref = Ref(**synth.MINI_UNET_CONFIG, **mc).state_dict()
-    spec = unet_param_spec(dict(synth.MINI_UNET_CONFIG), mc)
-    assert set(ref.keys()) == set(spec.keys()), (set(ref) ^ set(spec))  # module registration order differs, names do not
-    for k, v in ref.items():
-        assert tuple(v.shape) == tuple(spec[k][0]), k
-print("OK")
-''' % ROOT
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0 and "OK" in out.stdout, out.stderr[-2000:]
+    """Parameter names and shapes of the reference UNet's state_dict (recorded from the unmodified reference for three model configs of
+    the mini geometry: tests/golden/ref_unet_state_dict_shapes.json.gz) equal unet_param_spec's."""
+    ref_all = json.load(gzip.open(os.path.join(ROOT, "tests", "golden", "ref_unet_state_dict_shapes.json.gz")))
+    assert len(ref_all) == 3
+    for rec in ref_all.values():
+        spec = unet_param_spec(dict(synth.MINI_UNET_CONFIG), rec["model_config"])
+        ref = rec["shapes"]
+        assert set(ref) == set(spec), (set(ref) ^ set(spec))  # module registration order differs, names do not
+        for k, v in ref.items():
+            assert tuple(v) == tuple(spec[k][0]), k
 
 
 def test_alias_package_paths():
-    """The reference's dotted import paths (YAML `target:` strings, test_fatezero.py:24-30) resolve to the B200 classes."""
+    """The reference's dotted import paths (YAML `target:` strings, test_fatezero.py:24-30) resolve to the fatezero_b200 classes."""
     code = ("import video_diffusion.pipelines.p2p_ddim_spatial_temporal as p, video_diffusion.prompt_attention.attention_util as a, "
             "video_diffusion.models.unet_3d_condition as u, video_diffusion.prompt_attention.spatial_blend as sb; "
             "import fatezero_b200 as f; assert p.P2pDDIMSpatioTemporalPipeline is f.P2pDDIMSpatioTemporalPipeline; "

@@ -63,7 +63,7 @@ SELF_CASES = [
     (4, 4, 256, 4, 16, "prev_first"),
     (2, 2, 144, 4, 80, "prev_first"),
     (2, 2, 576, 2, 64, "mid"),
-    # TMEM-resident-P kernel (no hook, d <= 64, 128-key tiles): 1, 3, 5 and 10 key tiles, odd / even, one and two K/V frames
+    # no hook, d <= 64, multiples of 128 keys: 1, 3, 5 and 10 128-key blocks, odd / even, one and two K/V frames
     (2, 2, 128, 2, 40, "own"),
     (3, 3, 384, 2, 48, "mid"),
     (2, 2, 640, 1, 40, "own"),
@@ -97,8 +97,8 @@ def test_self_plain(BF, F_, S, heads, d, kind, report):
 
 @pytest.mark.parametrize("ramp", ["up", "down", "spike"])
 def test_self_plain_online_rescale(ramp, report):
-    """The hook-free kernel raises its reference maximum lazily (only when a 128-key tile exceeds it by 2^8) and then rescales O and
-    the row sum: key blocks with growing / shrinking / one spiking scale force that path (random inputs alone never trigger it)."""
+    """Key blocks with growing / shrinking / one spiking scale: the row maximum sits in a late, an early or a single 128-key block, which
+    random inputs alone never produce."""
     BF, F_, S, heads, d = 2, 2, 640, 2, 40
     q, k, v, vt = make_inputs(BF, S, S, BF, heads, d, seed=21, qscale=2.0)
     kk = k.float().reshape(BF, S, heads * d)
@@ -161,7 +161,7 @@ def make_xedit(mode, alpha, eq, a, mapper, M):
     return t.to(dev)
 
 
-# (1, 4096, 8, 40) / (8, 4096, 8, 40): the streaming cross-attention kernel with 2 / 11 query tiles per CTA (the step's own shape)
+# (1, 4096, 8, 40) / (8, 4096, 8, 40): the step's own text cross-attention shapes at the 64x64 latents
 @pytest.mark.parametrize("F_,S,heads,d", [(2, 64, 8, 160), (3, 256, 8, 40), (2, 1024, 8, 80), (2, 4096, 2, 40), (2, 144, 4, 16),
                                         (1, 4096, 8, 40), (8, 4096, 8, 40), (4, 1024, 8, 32)])
 def test_cross(F_, S, heads, d, report):

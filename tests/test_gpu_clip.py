@@ -1,4 +1,4 @@
-"""CLIP text encoder on the sm_100a kernels (fatezero_b200/clip.py) against transformers' CLIPTextModel (the module the reference calls at
+"""CLIP text encoder on the sm_90a kernels (fatezero_b200/clip.py) against transformers' CLIPTextModel (the module the reference calls at
 pipelines/stable_diffusion.py:230,279), same random-init weights, fp32 torch on the GPU as the checker.  Bound: fp16 storage through 12
 layers vs fp32 — measured value printed, bound 2x."""
 import pytest

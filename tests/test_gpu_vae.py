@@ -1,4 +1,4 @@
-"""VAE encode / decode on the sm_100a kernels (fatezero_b200/vae.py) against the fp32 torch restatement oracle/vae_oracle.py on the same
+"""VAE encode / decode on the sm_90a kernels (fatezero_b200/vae.py) against the fp32 torch restatement oracle/vae_oracle.py on the same
 name-keyed synthetic weights.  NOTE (DESIGN.md §5): that restatement is NOT pinned to the real diffusers package (absent offline), so this
 is parity of two independent restatements of the published AutoencoderKL; bounds are fp16-storage bounds, 2x the measured values."""
 import pytest

@@ -1,4 +1,4 @@
-"""Single attention configurations for ncu (S=4096 d=40 PLAIN by default). MODE=none|store|replace S=.. D=.."""
+"""Single attention configurations (S=4096 d=40 without a controller hook by default). MODE=none|store|replace S=.. D=.."""
 import os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -29,12 +29,3 @@ for _ in range(5): fn()
 e.record(); torch.cuda.synchronize()
 ms = s.elapsed_time(e) / 5
 print(dict(S=S, d=d, mode=mode, ms=ms, tflops=4 * BF * heads * S * S * len(si) * d / ms / 1e9))
-dbg = torch.zeros(32, dtype=torch.int64, device=dev)
-kw["dbg"] = dbg
-fn(); torch.cuda.synchronize()
-v = dbg.tolist()
-print("raw dbg: MMA", v[0:5], "WG A", v[8:16], "WG B", v[16:24], "QK issue: fence, mma, commit, tail", v[24:28])
-print("MMA thread : wait s_empty %d, ring_full(S) %d, p_full %d, ring_full(V) %d, total %d" % tuple(v[0:5]))
-for name, b in (("WG A", 8), ("WG B", 16)):
-    print(name, ": wait s_full(p1) %d, s_full(p2) %d, p_empty %d, bar1 %d, bar2 %d, o_full %d, end_pass2 %d, total %d" % tuple(v[b:b + 8]))
-print("pass-1 end at", v[24], " MMA warp: S-mma issue %d, S commits %d, PV-mma issue %d" % tuple(v[25:28]))

@@ -1,6 +1,6 @@
-"""Representative launches of the two tensor-core kernels for `ncu --set full` (see profiles/README.md):
+"""Representative launches of the two tensor-core kernels for `ncu --set full`:
   1) 3x3 conv 320->320 at 64x64, B*F=16     (tapgemm<160>, 9 taps)      2) linear 65536 x 960 x 320 (QKV, V^T epilogue off)
-  3) GEGLU linear 65536 x 2560 x 320         (tapgemm<256>)              4) ST-attention r=64 d=40 PLAIN
+  3) GEGLU linear 65536 x 2560 x 320         (tapgemm<256>)              4) ST-attention r=64 d=40 (no hook)
   5) ST-attention r=32 d=80 STORE            6) ST-attention r=32 d=80 REPLACE"""
 import os, sys
 import torch

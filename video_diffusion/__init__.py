@@ -1,5 +1,5 @@
 """Drop-in alias of the reference's `video_diffusion` import paths (hard-coded in its YAML configs and test_fatezero.py:24-30),
-backed by the B200-native implementation in `fatezero_b200`.  Only the hot-path surface of SURVEY.md §8(b) is provided."""
+backed by the H100-native implementation in `fatezero_b200`.  Only the hot-path surface of SURVEY.md §8(b) is provided."""
 
 
 def _extend_with_reference(pkg_path, pkg_file, sub):
