@@ -516,6 +516,10 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   if (a->row_mode == FZ_ATTN_BLEND) FZ_CHECK_ARG(a->mask, "fz_attention: BLEND needs a mask");
   if (a->row_mode == FZ_ATTN_CROSSEDIT) FZ_CHECK_ARG(a->xedit && a->n_slots == 1 && a->keys_per_slot <= 80, "fz_attention: CROSSEDIT needs tables, one slot, <= 80 keys");
   if (a->acc) FZ_CHECK_ARG(a->n_slots == 1 && a->acc_ld % 8 == 0, "fz_attention: running sum only for single-slot maps");
+  if (a->store || a->base)
+    FZ_CHECK_ARG(a->cache_ld > 0 && a->cache_ld % a->n_slots == 0 && a->cache_ld / a->n_slots >= a->keys_per_slot,
+                 "fz_attention: cache_ld=%lld must split into n_slots=%d runs of >= keys_per_slot=%d keys", a->cache_ld, a->n_slots,
+                 a->keys_per_slot);
   {
     uint64_t dims[4] = {(uint64_t)a->d, (uint64_t)a->heads, (uint64_t)a->S_q, (uint64_t)a->BF};
     uint64_t strides[3] = {(uint64_t)a->d, (uint64_t)a->ldq, (uint64_t)a->ldq * a->S_q};

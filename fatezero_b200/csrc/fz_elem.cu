@@ -911,7 +911,7 @@ static int launch_temporal_px(const void* qkv, void* out, int B, int HW, int hea
 }
 
 extern "C" int fz_temporal_attn_f16(const void* qkv, void* out, int B, int F, int HW, int heads, int d, float scale, cudaStream_t stream) {
-  FZ_CHECK_ARG(qkv && out && F <= kTaMaxF && d % 2 == 0, "fz_temporal_attn: F=%d d=%d unsupported", F, d);
+  FZ_CHECK_ARG(qkv && out && F >= 1 && F <= kTaMaxF && d % 2 == 0, "fz_temporal_attn: F=%d d=%d unsupported", F, d);
   if (d % 8 == 0 && d <= 320) {
     int hg = std::max(1, std::min(heads, 320 / d));  // heads per warp: 15 KB of q|k|v per (pixel, head group)
     while (heads % hg) --hg;
@@ -922,8 +922,11 @@ extern "C" int fz_temporal_attn_f16(const void* qkv, void* out, int B, int F, in
       default: break;
     }
   }
-  const int wpb = 8;
+  // up to 8 warps per block, as many as the per-block shared-memory limit holds (a 32-frame clip at d = 160 takes 34 KB per warp)
+  constexpr size_t kSmemBudget = 227 * 1024;
   const size_t per_warp = static_cast<size_t>(3 * F * d + F * F * 2) * sizeof(__half);
+  FZ_CHECK_ARG(per_warp <= kSmemBudget, "fz_temporal_attn: F=%d d=%d needs %zu B of shared memory per warp", F, d, per_warp);
+  const int wpb = static_cast<int>(std::min<size_t>(8, kSmemBudget / per_warp));
   const size_t smem = per_warp * wpb;
   static size_t configured = 0;
   if (smem > 48 * 1024 && smem > configured) {

@@ -398,6 +398,9 @@ static int fill_epilogue(TapGemmParams& p, const fz_epilogue_t* e, int M, int ge
   p.mode = e->mode;
   if (e->mode == FZ_EPI_GEGLU) {
     FZ_CHECK_ARG(gemm_cols % 2 == 0, "GEGLU needs an even number of GEMM columns");
+    // the GEGLU epilogue applies the bias only: any other term would be dropped without a trace
+    FZ_CHECK_ARG(!e->residual && !e->residual2 && !e->group_bias && !e->out_vt,
+                 "GEGLU epilogue takes no residual, group bias or V^T output");
     p.N = gemm_cols / 2;
   }
   if (e->out_vt) {

@@ -43,6 +43,7 @@ typedef struct fz_epilogue {
   const void* residual2;   /* second skip tensor (resnet shortcut next to the LoRA identity skip) or NULL           */
   long long ldr2;
   int mode;                /* FZ_EPI_GEGLU: columns [0,BN/2) x, [BN/2,BN) gate per tile -> x*gelu(gate)           */
+                           /*   (GEGLU takes the bias only: residuals, group_bias or out_vt are refused)         */
   int vt_col_start;        /* columns >= vt_col_start are stored transposed into out_vt (V^T for the PV GEMM)     */
   void* out_vt;            /* [M / vt_S, vt_heads, vt_d, vt_S] fp16 or NULL                                       */
   int vt_S, vt_d, vt_heads; /* row m = bf*vt_S + s  ->  out_vt[((bf*heads + h)*d + dd)*vt_ld + s]                  */
@@ -102,6 +103,7 @@ typedef struct fz_attn_args {
   void* store;                      /* cache slab written  [BF-edit_bf_start, heads, S_q, cache_ld] fp16             */
   const void* base;                 /* cache slab read     (same geometry)                                           */
   long long cache_ld;               /* n_slots*S_q for self maps; 80 for cross maps (77 keys padded to 16 bytes)     */
+                                    /*   must split into n_slots runs of cache_ld/n_slots >= keys_per_slot keys      */
   void* acc;       long long acc_ld;/* fp16 running sum slab or NULL (attention_store.py:95-101)                    */
   const float* xedit;               /* device table, see above                                                       */
   const float* mask;                /* device [BF-edit_bf_start, S_q], 1 = keep current row                          */
@@ -141,7 +143,7 @@ int fz_out_temporal_f32(const void* y, int ldy, float* eps, int B, int Co, int F
 /* y[n] = bias[n] + sum_k act(x[k]) W[n,k]; W fp16 (time embedding MLP and the 22 time_emb_proj rows, resnet.py:355) */
 int fz_rowvec_linear(const float* x, const void* W_f16, const float* bias, float* y, int N, int K, int silu_in, fz_stream_t stream);
 int fz_timestep_sinusoid(float t, float* out, int C0, int flip_sin_to_cos, float freq_shift, fz_stream_t stream);
-/* temporal attention over frames (models/attention.py:327-337): qkv [B*F*HW, 3C] -> out [B*F*HW, C] */
+/* temporal attention over frames (models/attention.py:327-337): qkv [B*F*HW, 3C] -> out [B*F*HW, C], 1 <= F <= 32 */
 int fz_temporal_attn_f16(const void* qkv, void* out, int B, int F, int HW, int heads, int d, float scale, fz_stream_t stream);
 /* x <- inversion step (p2p_ddim_spatial_temporal.py:150-161) */
 int fz_ddim_invert_step(float* x, const float* eps, long long n, float alpha_prev, float alpha_next, fz_stream_t stream);
