@@ -38,6 +38,19 @@ class AttnArgs(C.Structure):
     ]
 
 
+MAX_ATTN_GROUPS = 8
+
+
+class AttnGroup(C.Structure):
+    """fz_attn_group_t"""
+    _fields_ = [("row_mode", c_int), ("xedit", c_void_p), ("mask", c_void_p), ("acc", c_void_p)]
+
+
+class AttnGroups(C.Structure):
+    """fz_attn_groups_t"""
+    _fields_ = [("n_groups", c_int), ("g", AttnGroup * MAX_ATTN_GROUPS)]
+
+
 class P2PSeg(C.Structure):
     """fz_p2p_seg_t"""
     _fields_ = [("src", c_void_p), ("src_pitch", c_ll), ("dst", c_void_p), ("dst_pitch", c_ll), ("rows", c_int), ("row_bytes", c_int),
@@ -58,8 +71,11 @@ SIGNATURES = {
     "fz_tconv3_f16": [c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p, c_int, C.POINTER(Epilogue), c_void_p, c_ll, c_int, c_void_p],
     "fz_tconv3_halo_f16": [c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p, c_int, C.POINTER(Epilogue), c_void_p, c_ll, c_int, c_void_p],
     "fz_attention_f16": [C.POINTER(AttnArgs), c_void_p],
+    "fz_attention_grouped_f16": [C.POINTER(AttnArgs), C.POINTER(AttnGroups), c_void_p],
     "fz_groupnorm_nhwc_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p,
                               c_void_p],
+    "fz_groupnorm_batched_nhwc_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int,
+                                      c_void_p, c_void_p],
     "fz_groupnorm_stats_f16": [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
     "fz_groupnorm_apply_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p,
                                c_void_p],
@@ -74,6 +90,8 @@ SIGNATURES = {
     "fz_temporal_attn_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p],
     "fz_ddim_invert_step": [c_void_p, c_void_p, c_ll, c_float, c_float, c_void_p],
     "fz_cfg_ddim_step": [c_void_p, c_void_p, c_ll, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p],
+    "fz_cfg_ddim_step_batched": [c_void_p, c_void_p, c_int, c_ll, c_float, c_float, c_float, c_void_p, C.POINTER(c_void_p),
+                                 C.POINTER(c_void_p), C.POINTER(c_int), c_ll, c_void_p],
     "fz_blend_mask": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(c_float), c_float, c_int, c_int,
                       c_void_p, c_void_p],
     "fz_p2p_alloc": [c_ll, C.POINTER(c_void_p)],
@@ -96,7 +114,7 @@ SIGNATURES = {
 _lib = None
 launch_count = 0     # C-ABI compute calls issued
 kernel_launches = 0  # kernels of this library launched (bench.py reports the delta over its timed region)
-KERNELS_PER_CALL = {"fz_groupnorm_nhwc_f16": 2, "fz_p2p_alloc": 0, "fz_p2p_free": 0, "fz_p2p_export": 0, "fz_p2p_import": 0,
+KERNELS_PER_CALL = {"fz_groupnorm_nhwc_f16": 2, "fz_groupnorm_batched_nhwc_f16": 2, "fz_p2p_alloc": 0, "fz_p2p_free": 0, "fz_p2p_export": 0, "fz_p2p_import": 0,
                     "fz_p2p_unimport": 0, "fz_init": 0}  # stats + apply (plus one memset); every other entry point launches one kernel
 
 

@@ -571,6 +571,114 @@ class AttentionReweight(AttentionControlEdit):
         return mode, mapper, a, M, self.equalizer.reshape(-1)
 
 
+class AttentionControlEditBatch:
+    """K edit controllers of ONE inverted clip driven through one batched edit pass (CFG batch [uncond_1..K ; cond_1..K]).
+
+    Every child is asked exactly what it would be asked in its own single-prompt pass (a CFG batch of 2 at `frames` frames), so its
+    position counters, tables, masks and running sums evolve as in that pass; the answers are merged into one grouped attention launch
+    (fz_attention_grouped_f16: child k owns rows [(K + k) F, (K + k + 1) F)), and a child that answers None becomes a NONE group.  The
+    children must edit against the same inversion store with the same step count and store indexing."""
+
+    def __init__(self, edits: List[AttentionControlEdit]):
+        edits = list(edits)
+        if not edits or len(edits) > _lib.MAX_ATTN_GROUPS:
+            raise ValueError(f"AttentionControlEditBatch: 1..{_lib.MAX_ATTN_GROUPS} edit controllers, got {len(edits)}")
+        c0 = edits[0]
+        for e in edits[1:]:
+            if e.additional_attention_store is not c0.additional_attention_store:
+                raise ValueError("AttentionControlEditBatch: every edit must read the same additional_attention_store")
+            if e.num_steps != c0.num_steps or bool(e.use_inversion_attention) != bool(c0.use_inversion_attention):
+                raise ValueError("AttentionControlEditBatch: every edit must share num_steps and use_inversion_attention")
+        store = c0.additional_attention_store
+        if any(getattr(e, "disk_store", False) for e in edits) or getattr(store, "disk_store", False) or getattr(store, "host_spill", False):
+            raise NotImplementedError("AttentionControlEditBatch: disk_store / host_spill stores are edited one prompt at a time")
+        self.edits = edits
+        self.prompt_groups = len(edits)
+        self.LOW_RESOURCE = False
+        self.num_att_layers = -1
+        self._frames = None
+
+    # ---- state shared with the children --------------------------------------------------------------------------------
+    @property
+    def cur_step(self) -> int:
+        return self.edits[0].cur_step
+
+    @property
+    def additional_attention_store(self):
+        return self.edits[0].additional_attention_store
+
+    def __setattr__(self, name, value):
+        object.__setattr__(self, name, value)
+        if name == "num_att_layers":  # register_attention_control sets it on whatever object it is given: pass it on
+            for e in self.__dict__.get("edits", []):
+                e.num_att_layers = value
+
+    # ---- fused-kernel protocol ------------------------------------------------------------------------------------------
+    def begin_forward(self, batch, frames):
+        if batch != 2 * self.prompt_groups:
+            raise RuntimeError(f"AttentionControlEditBatch: expected a CFG batch of 2 x {self.prompt_groups} prompts, got {batch}")
+        self._frames = frames
+        for e in self.edits:
+            e.begin_forward(2, frames)
+
+    def _merge(self, answers: List[Optional[dict]], frames: int) -> Optional[dict]:
+        if self.prompt_groups == 1:
+            return answers[0]
+        live = [a for a in answers if a is not None]
+        if not live:
+            return None
+        base, cache_ld = live[0]["base"], live[0]["cache_ld"]
+        for a in live[1:]:
+            if a["base"].data_ptr() != base.data_ptr() or a["cache_ld"] != cache_ld or a["base"].shape != base.shape:
+                raise RuntimeError("AttentionControlEditBatch: the edits disagree on the cached inversion map of this layer")
+        for a in live:
+            if a["edit_bf_start"] != frames:
+                raise RuntimeError("AttentionControlEditBatch: an edit asked for rows outside its conditional half")
+        groups = [dict(row_mode=_lib.ATTN_NONE) if a is None else
+                  dict(row_mode=a["row_mode"], mask=a.get("mask"), acc=a.get("acc"), xedit=a.get("xedit")) for a in answers]
+        return dict(edit_bf_start=self.prompt_groups * frames, base=base, cache_ld=cache_ld, groups=groups)
+
+    def self_attn_args(self, place, S, T, heads, nb, frames):
+        return self._merge([e.self_attn_args(place, S, T, heads, 2 * frames, frames) for e in self.edits], frames)
+
+    def cross_attn_args(self, place, S, heads, nb, frames):
+        return self._merge([e.cross_attn_args(place, S, heads, 2 * frames, frames) for e in self.edits], frames)
+
+    def latent_blend_args(self, h: int, w: int) -> List[Optional[dict]]:
+        return [e.latent_blend_args(h, w) for e in self.edits]
+
+    def step_callback(self, x_t, blend_fused: bool = False):
+        for k, e in enumerate(self.edits):
+            e.step_callback(x_t[k:k + 1], blend_fused=blend_fused)
+        return x_t
+
+    def reset(self):
+        for e in self.edits:
+            e.reset()
+
+    # ---- CUDA-graph replay support: composed from the children's --------------------------------------------------------------
+    def graph_signature(self):
+        sigs = [e.graph_signature() for e in self.edits]
+        if any(s is None for s in sigs):
+            return None
+        # the last element is the inversion store's plan id (shared by the children), as for a single edit
+        return ("edit_batch", tuple(s[:-1] for s in sigs), sigs[0][-1])
+
+    def prepare_tables(self, device):
+        for e in self.edits:
+            e.prepare_tables(device)
+
+    def load_tables_from(self, other: "AttentionControlEditBatch"):
+        for mine, theirs in zip(self.edits, other.edits):
+            mine.load_tables_from(theirs)
+
+    def adopt_from(self, tmpl: "AttentionControlEditBatch"):
+        if tmpl is self:
+            return
+        for mine, theirs in zip(self.edits, tmpl.edits):
+            mine.adopt_from(theirs)
+
+
 def get_equalizer(text: str, word_select, values, tokenizer=None):
     return tables.get_equalizer(text, word_select, values, tokenizer)
 

@@ -11,6 +11,8 @@
 //              (attention_util.py:80-92 without mask)
 //   BLEND      edit, self-attention with a per-(frame,pixel) mask: rows with mask==0 take the cached row (:86-88)
 //   CROSSEDIT  edit, cross-attention: Refine gather / Replace 77x77 / Reweight / alpha-lerp in registers (:130-131,213-253,282-286)
+// The hook is chosen per row group (fz_attention_grouped_f16: K prompts of one clip in one CFG batch, each group with its own mode, mask,
+// running sum and edit tables, all reading one cached map); fz_attention_f16 is the one-group case.
 // Hooked rows take two passes over the keys (max and sum first, then probabilities): the normalised fp16 P the reference stores and
 // multiplies is reproduced exactly at its rounding point.  Rows that are neither stored nor edited take ONE pass with a running reference
 // maximum (online softmax: p = exp2(s c - m_ref c) rounded to fp16 for PV, fp32 row sum l, O / l at the end; m_ref is raised, and O, l
@@ -31,7 +33,9 @@
 namespace fz {
 
 constexpr int kMaxSlots = 4;
-constexpr int kMaxBF = 64;
+constexpr int kMaxBF = 64;          // fz_attention_f16
+constexpr int kMaxBFGrouped = 128;  // fz_attention_grouped_f16: 8 prompts x CFG 2 x 8 frames
+constexpr int kMaxGroups = FZ_ATTN_MAX_GROUPS;
 constexpr int kAtomBytes = 128 * 128;  // 128 rows x 64 fp16
 constexpr int kHalfAtom = 64 * 128;    // one warpgroup's 64 rows
 constexpr int kMaxStages = 12;
@@ -49,21 +53,28 @@ struct AttnParams {
   int heads, F, BF;
   int ring_stages, ring_stage_bytes;
   float scale_log2;     // scale * log2(e)
-  int src_index[kMaxSlots][kMaxBF];  // K/V source row (frame or text batch) per slot and query frame
-  // controller
-  int edit_bf_start;    // rows bf >= edit_bf_start get row_mode; cache frame = bf - edit_bf_start
-  int row_mode;         // FZ_ATTN_*
-  __half* acc;          // running sum [Fc, heads, S_q, acc_ld] fp16 or null (cross maps)
+  int src_index[kMaxSlots][kMaxBFGrouped];  // K/V source row (frame or text batch) per slot and query frame
+  // controller: rows bf >= edit_bf_start form n_groups groups of group_rows rows; row bf belongs to group
+  // g = (bf - edit_bf_start) / group_rows and reads cache frame fc = (bf - edit_bf_start) % group_rows of the shared base slab
+  int edit_bf_start;
+  int group_rows;       // Fc: rows per group (the base / store slabs are [Fc, heads, S_q, cache_ld])
+  int n_groups;
+  unsigned char row_group[kMaxBFGrouped];  // g of every row (0 for the rows before edit_bf_start)
+  int has_base;         // some group is REPLACE / BLEND: the shared-memory plan holds the two cached-P tiles
+  int g_row_mode[kMaxGroups];      // FZ_ATTN_* per group
+  __half* g_acc[kMaxGroups];       // running sum [Fc, heads, S_q, acc_ld] fp16 or null (cross maps), per group
+  const float* g_xedit[kMaxGroups];  // CROSSEDIT tables in device memory (fz_cross_edit_t layout), per group
+  const float* g_mask[kMaxGroups];   // BLEND: [Fc, S_q] 1 = keep current row, 0 = take cached row, per group
   long long acc_ld;
   const __half* base_rows;  // CROSSEDIT: cached source map [Fc, heads, S_q, base_ld]
   long long base_ld;
-  const float* xedit;   // CROSSEDIT tables in device memory: see fz_cross_edit_t
-  const float* mask;    // BLEND: [Fc, S_q] 1 = keep current row, 0 = take cached row
   __half* out;          // [BF*S_q, ldo], this head's columns start at head*d
   long long ldo;
   int causal;           // key n visible to query s only if n <= s
   int masked;           // keys_per_slot % 64 != 0 or causal: scores outside the valid keys are set to -inf
 };
+// a __grid_constant__ parameter block must stay within the classic 4 KiB kernel-parameter space
+static_assert(sizeof(AttnParams) <= 4096, "AttnParams exceeds the 4 KiB kernel-parameter limit");
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
@@ -123,9 +134,10 @@ __global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ At
   const int q0 = blockIdx.x * 128;
   const int head = blockIdx.y;
   const int bf = blockIdx.z;
-  const bool edited = bf >= p.edit_bf_start && p.row_mode != FZ_ATTN_NONE;
-  const int row_mode = edited ? p.row_mode : FZ_ATTN_NONE;
-  const int fc = bf - p.edit_bf_start;
+  const int grp = p.row_group[bf];
+  const int fc = bf - p.edit_bf_start - grp * p.group_rows;
+  const bool edited = bf >= p.edit_bf_start && p.g_row_mode[grp] != FZ_ATTN_NONE;
+  const int row_mode = edited ? p.g_row_mode[grp] : FZ_ATTN_NONE;
   const bool replace = row_mode == FZ_ATTN_REPLACE;
   const bool blend = row_mode == FZ_ATTN_BLEND;
   const bool exact = row_mode != FZ_ATTN_NONE;  // pass 1 accumulates the sum, pass 2 emits normalised probabilities
@@ -134,8 +146,7 @@ __global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ At
   uint8_t* s_ring = s_q + p.nd * kAtomBytes;
   uint8_t* s_p = s_ring + p.ring_stages * p.ring_stage_bytes;  // [warpgroup][2] x 8 KiB
   uint8_t* s_base = s_p + 4 * kHalfAtom;                       // 2 x 16 KiB (REPLACE / BLEND only)
-  const bool has_base = p.row_mode == FZ_ATTN_REPLACE || p.row_mode == FZ_ATTN_BLEND;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_base + (has_base ? 2 * kAtomBytes : 0));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_base + (p.has_base ? 2 * kAtomBytes : 0));
   uint64_t* ring_full = bars;                   // [kMaxStages]
   uint64_t* ring_empty = bars + kMaxStages;     // [kMaxStages]
   uint64_t* q_full = bars + 2 * kMaxStages;
@@ -291,13 +302,14 @@ __global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ At
       }
     }
     float inv_l[2], mb2[2], mrow[2];
-    const float* xe = p.xedit;
-    const bool row_ops = row_mode == FZ_ATTN_CROSSEDIT || (p.acc && edited);
+    // the group's acc / xedit pointers are re-read from the parameter block where they are used (keeping them live spills at d > 128)
+    const bool has_acc = edited && p.g_acc[grp] != nullptr;
+    const bool row_ops = row_mode == FZ_ATTN_CROSSEDIT || has_acc;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       inv_l[h] = exact ? 1.0f / quad_sum(l_run[h]) : 1.0f;
       mb2[h] = exact ? m_run[h] * sc2 : 0.f;
-      mrow[h] = blend ? p.mask[static_cast<long long>(fc) * p.S_q + min(q[h], p.S_q - 1)] : 1.f;
+      mrow[h] = blend ? p.g_mask[grp][static_cast<long long>(fc) * p.S_q + min(q[h], p.S_q - 1)] : 1.f;
       l_run[h] = 0.f;
     }
     // ------------------------ pass 2 (the only pass of un-hooked rows): probabilities -> P tile (-> cache) -> O += P V ------------------------
@@ -341,8 +353,8 @@ __global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ At
         for (int h = 0; h < 2; ++h) {
           // key index n = ai.k0 + 8 i + c_base + j (single slot).  cur = fp16(p); optional running sum; optional edit (in fp32, one rounding)
           const long long rbase = ((static_cast<long long>(fc) * p.heads + head) * p.S_q + min(q[h], p.S_q - 1));
-          if (p.acc && row_ok[h]) {
-            __half* ap = p.acc + rbase * p.acc_ld;
+          if (has_acc && row_ok[h]) {
+            __half* ap = p.g_acc[grp] + rbase * p.acc_ld;
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               const int n = ai.k0 + 8 * i + c_base;
@@ -355,6 +367,7 @@ __global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ At
           }
           if (row_mode == FZ_ATTN_CROSSEDIT) {
             const __half* brow = p.base_rows + rbase * p.base_ld;
+            const float* xe = p.g_xedit[grp];
             const int xmode = static_cast<int>(xe[0]);  // 0 refine, 1 replace
             const float* x_alpha = xe + 8;              // [80] cross_replace_alpha of this step
             const float* x_eq = xe + 8 + 80;            // [80] equalizer (1 when absent)
@@ -486,13 +499,9 @@ static int encode_cache_map(CUtensorMap* tm, const void* base, int keys_ld_slot,
   return encode_tmap_f16(tm, base, 5, dims, strides, box, true);
 }
 
-extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
-  if (int rc = check_single_device()) return rc;
-  FZ_CHECK_ARG(a && a->q && a->k && a->vt && a->out, "fz_attention: null pointer");
-  FZ_CHECK_ARG(a->d % 8 == 0 && a->d >= 8 && a->d <= 192, "fz_attention: head dim %d unsupported", a->d);
-  FZ_CHECK_ARG(a->n_slots >= 1 && a->n_slots <= kMaxSlots && a->BF <= kMaxBF, "fz_attention: n_slots=%d BF=%d unsupported", a->n_slots, a->BF);
-  FZ_CHECK_ARG(a->ldq % 8 == 0 && a->ldk % 8 == 0 && a->vt_ld % 8 == 0 && a->ldo % 8 == 0, "fz_attention: leading dims must be multiples of 8");
-  FZ_CHECK_ARG(a->keys_per_slot >= 1 && a->keys_per_slot <= a->vt_ld, "fz_attention: keys_per_slot > vt_ld");
+// One launcher for both entries.  `g` carries the controller hook per row group; rows [edit_bf_start, BF) form g->n_groups groups of
+// group_rows rows, all reading the same base slab [group_rows, heads, S_q, cache_ld].
+static int attention_launch(const fz_attn_args_t* a, const fz_attn_groups_t* g, int group_rows, cudaStream_t stream) {
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.S_q = a->S_q; p.keys_per_slot = a->keys_per_slot; p.n_slots = a->n_slots;
@@ -501,21 +510,36 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   p.scale_log2 = a->scale * 1.4426950408889634f;
   for (int s = 0; s < a->n_slots; ++s)
     for (int i = 0; i < a->BF; ++i) p.src_index[s][i] = a->src_index[s * a->BF + i];
-  p.edit_bf_start = a->edit_bf_start; p.row_mode = a->row_mode;
-  p.acc = static_cast<__half*>(a->acc); p.acc_ld = a->acc_ld;
+  p.edit_bf_start = a->edit_bf_start;
+  p.group_rows = std::max(1, group_rows);
+  p.n_groups = g->n_groups;
+  for (int i = std::max(0, a->edit_bf_start); i < a->BF; ++i) p.row_group[i] = static_cast<unsigned char>((i - a->edit_bf_start) / p.group_rows);
+  bool any_store = false, any_base = false, any_self_base = false, any_hook = false;
+  for (int k = 0; k < g->n_groups; ++k) {
+    const fz_attn_group_t& gr = g->g[k];
+    FZ_CHECK_ARG(gr.row_mode >= FZ_ATTN_NONE && gr.row_mode <= FZ_ATTN_CROSSEDIT, "fz_attention: group %d: row_mode %d unknown", k, gr.row_mode);
+    p.g_row_mode[k] = gr.row_mode;
+    p.g_acc[k] = static_cast<__half*>(gr.acc);
+    p.g_xedit[k] = gr.xedit;
+    p.g_mask[k] = gr.mask;
+    any_store |= gr.row_mode == FZ_ATTN_STORE;
+    any_self_base |= gr.row_mode == FZ_ATTN_REPLACE || gr.row_mode == FZ_ATTN_BLEND;
+    any_base |= gr.row_mode == FZ_ATTN_REPLACE || gr.row_mode == FZ_ATTN_BLEND || gr.row_mode == FZ_ATTN_CROSSEDIT;
+    any_hook |= gr.row_mode != FZ_ATTN_NONE || gr.acc != nullptr;
+    if (gr.row_mode == FZ_ATTN_BLEND) FZ_CHECK_ARG(gr.mask, "fz_attention: BLEND needs a mask");
+    if (gr.row_mode == FZ_ATTN_CROSSEDIT) FZ_CHECK_ARG(gr.xedit && a->n_slots == 1 && a->keys_per_slot <= 80, "fz_attention: CROSSEDIT needs tables, one slot, <= 80 keys");
+    if (gr.acc) FZ_CHECK_ARG(a->n_slots == 1 && a->acc_ld % 8 == 0, "fz_attention: running sum only for single-slot maps");
+  }
+  p.has_base = any_self_base;
+  p.acc_ld = a->acc_ld;
   p.base_rows = static_cast<const __half*>(a->base); p.base_ld = a->cache_ld;
-  p.xedit = a->xedit; p.mask = a->mask;
   p.out = static_cast<__half*>(a->out); p.ldo = a->ldo;
   p.causal = a->causal;
   p.masked = a->causal || a->keys_per_slot % 64 != 0;
-  if (a->causal) FZ_CHECK_ARG(a->n_slots == 1 && a->row_mode == FZ_ATTN_NONE && !a->acc, "fz_attention: causal masking needs one slot and no controller hook");
-  const int Fc = a->BF - a->edit_bf_start;
-  if (a->row_mode == FZ_ATTN_STORE) FZ_CHECK_ARG(a->store, "fz_attention: STORE needs a cache slab");
-  if (a->row_mode == FZ_ATTN_REPLACE || a->row_mode == FZ_ATTN_BLEND || a->row_mode == FZ_ATTN_CROSSEDIT)
-    FZ_CHECK_ARG(a->base, "fz_attention: REPLACE/BLEND/CROSSEDIT need the cached source map");
-  if (a->row_mode == FZ_ATTN_BLEND) FZ_CHECK_ARG(a->mask, "fz_attention: BLEND needs a mask");
-  if (a->row_mode == FZ_ATTN_CROSSEDIT) FZ_CHECK_ARG(a->xedit && a->n_slots == 1 && a->keys_per_slot <= 80, "fz_attention: CROSSEDIT needs tables, one slot, <= 80 keys");
-  if (a->acc) FZ_CHECK_ARG(a->n_slots == 1 && a->acc_ld % 8 == 0, "fz_attention: running sum only for single-slot maps");
+  if (a->causal) FZ_CHECK_ARG(a->n_slots == 1 && !any_hook, "fz_attention: causal masking needs one slot and no controller hook");
+  const int Fc = group_rows;
+  if (any_store) FZ_CHECK_ARG(a->store, "fz_attention: STORE needs a cache slab");
+  if (any_base) FZ_CHECK_ARG(a->base, "fz_attention: REPLACE/BLEND/CROSSEDIT need the cached source map");
   if (a->store || a->base)
     FZ_CHECK_ARG(a->cache_ld > 0 && a->cache_ld % a->n_slots == 0 && a->cache_ld / a->n_slots >= a->keys_per_slot,
                  "fz_attention: cache_ld=%lld must split into n_slots=%d runs of >= keys_per_slot=%d keys", a->cache_ld, a->n_slots,
@@ -544,15 +568,14 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   } else {
     p.tmStore = p.tmQ;
   }
-  if (a->base && a->row_mode != FZ_ATTN_CROSSEDIT) {
+  if (a->base && any_self_base) {
     if (int rc = encode_cache_map(&p.tmBase, a->base, (int)(a->cache_ld / a->n_slots), a->n_slots, a->S_q, a->heads, Fc, a->cache_ld)) return rc;
   } else {
     p.tmBase = p.tmQ;
   }
   // shared memory plan: Q + ring + 4 half P tiles (+ 2 base tiles) + barriers
-  const bool has_base = a->row_mode == FZ_ATTN_REPLACE || a->row_mode == FZ_ATTN_BLEND;
   const int stage_bytes = p.nd * 64 * 128;
-  const int fixed = p.nd * kAtomBytes + 4 * kHalfAtom + (has_base ? 2 * kAtomBytes : 0) + 1024 + 512;
+  const int fixed = p.nd * kAtomBytes + 4 * kHalfAtom + (p.has_base ? 2 * kAtomBytes : 0) + 1024 + 512;
   int stages = kMaxStages;
   while (stages > 2 && fixed + stages * stage_bytes > 227 * 1024) --stages;
   FZ_CHECK_ARG(fixed + stages * stage_bytes <= 227 * 1024, "fz_attention: shared memory plan does not fit (d=%d)", a->d);
@@ -570,4 +593,37 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   FZ_CUDA(launch_pdl(kernel, grid, dim3(288), smem, stream, p));
   FZ_CUDA(cudaGetLastError());
   return FZ_OK;
+}
+
+static int check_common(const fz_attn_args_t* a, int max_bf) {
+  if (int rc = check_single_device()) return rc;
+  FZ_CHECK_ARG(a && a->q && a->k && a->vt && a->out, "fz_attention: null pointer");
+  FZ_CHECK_ARG(a->d % 8 == 0 && a->d >= 8 && a->d <= 192, "fz_attention: head dim %d unsupported", a->d);
+  FZ_CHECK_ARG(a->n_slots >= 1 && a->n_slots <= kMaxSlots && a->BF <= max_bf, "fz_attention: n_slots=%d BF=%d unsupported", a->n_slots, a->BF);
+  FZ_CHECK_ARG(a->ldq % 8 == 0 && a->ldk % 8 == 0 && a->vt_ld % 8 == 0 && a->ldo % 8 == 0, "fz_attention: leading dims must be multiples of 8");
+  FZ_CHECK_ARG(a->keys_per_slot >= 1 && a->keys_per_slot <= a->vt_ld, "fz_attention: keys_per_slot > vt_ld");
+  return FZ_OK;
+}
+
+extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
+  if (int rc = check_common(a, kMaxBF)) return rc;
+  fz_attn_groups_t g;
+  memset(&g, 0, sizeof(g));
+  g.n_groups = 1;
+  g.g[0].row_mode = a->row_mode;
+  g.g[0].xedit = a->xedit;
+  g.g[0].mask = a->mask;
+  g.g[0].acc = a->acc;
+  return attention_launch(a, &g, a->BF - a->edit_bf_start, stream);
+}
+
+extern "C" int fz_attention_grouped_f16(const fz_attn_args_t* a, const fz_attn_groups_t* g, cudaStream_t stream) {
+  if (int rc = check_common(a, kMaxBFGrouped)) return rc;
+  FZ_CHECK_ARG(g && g->n_groups >= 1 && g->n_groups <= kMaxGroups, "fz_attention_grouped: n_groups=%d unsupported (1..%d)", g ? g->n_groups : 0,
+               kMaxGroups);
+  FZ_CHECK_ARG(a->F >= 1 && a->edit_bf_start >= 0 && a->BF - a->edit_bf_start == g->n_groups * a->F,
+               "fz_attention_grouped: BF - edit_bf_start = %d rows must be n_groups * F = %d * %d", a->BF - a->edit_bf_start, g->n_groups, a->F);
+  for (int k = 0; k < g->n_groups; ++k)
+    FZ_CHECK_ARG(g->g[k].row_mode != FZ_ATTN_STORE, "fz_attention_grouped: group %d: STORE is not a grouped mode", k);
+  return attention_launch(a, g, a->F, stream);
 }

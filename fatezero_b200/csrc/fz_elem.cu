@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 
 #include "../../include/fatezero_b200.h"
 
@@ -650,20 +651,31 @@ __global__ void ddim_invert_kernel(float* __restrict__ x, const float* __restric
   }
 }
 
-// eps2 = [uncond | cond] each n elements. mask (optional): [F*H*W] floats per frame pixel, broadcast over channels.
-__global__ void cfg_ddim_kernel(float* __restrict__ x, const float* __restrict__ eps2, long long n, float guidance, float sqrt_a_t,
+// K items of n_item elements: x [K, n_item], eps2 = [uncond_1..K | cond_1..K]. mask (optional, per item): [F*H*W] floats per frame pixel,
+// broadcast over channels; x_inv [n_item] is shared by the items.
+constexpr int kCfgMaxItems = 8;
+struct CfgItems {
+  const float* mask_a[kCfgMaxItems];
+  const float* mask_b[kCfgMaxItems];
+  int apply_blend[kCfgMaxItems];
+};
+
+__global__ void cfg_ddim_kernel(float* __restrict__ x, const float* __restrict__ eps2, int K, long long n_item, float guidance, float sqrt_a_t,
                                 float sqrt_1m_a_t, float sqrt_a_prev, float sqrt_1m_a_prev, const float* __restrict__ x_inv,
-                                const float* __restrict__ mask_a, const float* __restrict__ mask_b, long long fhw, int apply_blend) {
+                                const __grid_constant__ CfgItems items, long long fhw) {
+  const long long n = static_cast<long long>(K) * n_item;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float eu = eps2[i], ec = eps2[n + i];
     const float e = eu + guidance * (ec - eu);
     const float x0 = (x[i] - sqrt_1m_a_t * e) / sqrt_a_t;
     float xn = sqrt_a_prev * x0 + sqrt_1m_a_prev * e;
-    if (apply_blend) {
-      const long long q = i % fhw;
-      float m = mask_a[q];
-      if (mask_b) m = fmaxf(m, mask_b[q]);
-      const float xi = x_inv[i];
+    const int k = K == 1 ? 0 : static_cast<int>(i / n_item);
+    if (items.apply_blend[k]) {
+      const long long j = i - k * n_item;
+      const long long q = j % fhw;
+      float m = items.mask_a[k][q];
+      if (items.mask_b[k]) m = fmaxf(m, items.mask_b[k][q]);
+      const float xi = x_inv[j];
       xn = xi + m * (xn - xi);
     }
     x[i] = xn;
@@ -753,15 +765,16 @@ static inline int grid_for(long long total, int threads) {
 using namespace fz;
 
 // which = 1: statistics only, 2: apply only (image_sums supplied by the caller), 3: both
+// geometry_images: the number of images the chunking is planned for (NB, or the images of one item of a batched edit)
 static int groupnorm_impl(int which, const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, int count_frames,
                           const float* gamma, const float* beta, float eps, int silu, void* workspace_f64, const void* sums_in,
-                          cudaStream_t stream) {
+                          cudaStream_t stream, int geometry_images) {
   if (int rc = check_single_device()) return rc;
   FZ_CHECK_ARG(C % 8 == 0 && C % groups == 0 && groups <= 64, "fz_groupnorm: C=%d groups=%d unsupported", C, groups);
   FZ_CHECK_ARG(frames_per_stat >= 1 && NB % frames_per_stat == 0, "fz_groupnorm: NB %% frames_per_stat != 0");
   int TX, slots, ppc, chunks, ppc_apply, chunks_apply;
-  gn_geometry(C, HW, NB, 2, &TX, &slots, &ppc, &chunks);              // statistics: few fat CTAs (amortise the reduction tail)
-  gn_geometry(C, HW, NB, 4, &TX, &slots, &ppc_apply, &chunks_apply);  // apply: one full wave of 4 CTAs per SM
+  gn_geometry(C, HW, geometry_images, 2, &TX, &slots, &ppc, &chunks);              // statistics: few fat CTAs (amortise the reduction tail)
+  gn_geometry(C, HW, geometry_images, 4, &TX, &slots, &ppc_apply, &chunks_apply);  // apply: one full wave of 4 CTAs per SM
   FZ_CHECK_ARG(slots <= kGnMaxSlots, "fz_groupnorm: C=%d too large", C);
   FZ_CHECK_ARG(static_cast<size_t>(NB) * chunks * groups * sizeof(float2) <= kGnStatsOffset && NB <= 256, "fz_groupnorm: workspace (1 MiB) too small");
   const int TY = kGnThreads / TX;
@@ -799,21 +812,33 @@ static int groupnorm_impl(int which, const void* x, void* y, int NB, int HW, int
 extern "C" int fz_groupnorm_nhwc_f16(const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, const float* gamma,
                                      const float* beta, float eps, int silu, void* workspace_f64, cudaStream_t stream) {
   FZ_CHECK_ARG(x && y && gamma && beta && workspace_f64, "fz_groupnorm: null pointer");
-  return groupnorm_impl(3, x, y, NB, HW, C, groups, frames_per_stat, frames_per_stat, gamma, beta, eps, silu, workspace_f64, nullptr, stream);
+  return groupnorm_impl(3, x, y, NB, HW, C, groups, frames_per_stat, frames_per_stat, gamma, beta, eps, silu, workspace_f64, nullptr, stream,
+                        NB);
+}
+
+extern "C" int fz_groupnorm_batched_nhwc_f16(const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat,
+                                             int images_per_item, const float* gamma, const float* beta, float eps, int silu,
+                                             void* workspace_f64, cudaStream_t stream) {
+  FZ_CHECK_ARG(x && y && gamma && beta && workspace_f64, "fz_groupnorm: null pointer");
+  FZ_CHECK_ARG(images_per_item >= 1 && NB % images_per_item == 0 && images_per_item % frames_per_stat == 0,
+               "fz_groupnorm_batched: images_per_item=%d must divide NB=%d and be a multiple of frames_per_stat=%d", images_per_item, NB,
+               frames_per_stat);
+  return groupnorm_impl(3, x, y, NB, HW, C, groups, frames_per_stat, frames_per_stat, gamma, beta, eps, silu, workspace_f64, nullptr, stream,
+                        images_per_item);
 }
 
 // Frame-sharded GroupNorm (SURVEY.md 8(e)): statistics and apply as separate calls so that the (sum, sumsq) of the frames held by other
 // GPUs can be all-reduced in between.  fz_groupnorm_stats_f16 leaves float2 sums[NB][groups] at workspace + 768 KiB.
 extern "C" int fz_groupnorm_stats_f16(const void* x, int NB, int HW, int C, int groups, void* workspace_f64, cudaStream_t stream) {
   FZ_CHECK_ARG(x && workspace_f64, "fz_groupnorm_stats: null pointer");
-  return groupnorm_impl(1, x, nullptr, NB, HW, C, groups, 1, 1, nullptr, nullptr, 0.f, 0, workspace_f64, nullptr, stream);
+  return groupnorm_impl(1, x, nullptr, NB, HW, C, groups, 1, 1, nullptr, nullptr, 0.f, 0, workspace_f64, nullptr, stream, NB);
 }
 
 extern "C" int fz_groupnorm_apply_f16(const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, int count_frames,
                                       const float* gamma, const float* beta, float eps, int silu, const void* image_sums,
                                       cudaStream_t stream) {
   FZ_CHECK_ARG(x && y && gamma && beta && image_sums && count_frames >= frames_per_stat, "fz_groupnorm_apply: bad arguments");
-  return groupnorm_impl(2, x, y, NB, HW, C, groups, frames_per_stat, count_frames, gamma, beta, eps, silu, nullptr, image_sums, stream);
+  return groupnorm_impl(2, x, y, NB, HW, C, groups, frames_per_stat, count_frames, gamma, beta, eps, silu, nullptr, image_sums, stream, NB);
 }
 
 extern "C" int fz_layernorm_f16(const void* x, void* y, long long M, int C, const float* gamma, const float* beta, float eps,
@@ -948,14 +973,40 @@ extern "C" int fz_ddim_invert_step(float* x, const float* eps, long long n, floa
   return FZ_OK;
 }
 
+static int cfg_ddim_launch(float* x, const float* eps2, int K, long long n_item, float guidance, float a_t, float a_prev, const float* x_inv,
+                           const CfgItems& items, long long fhw, cudaStream_t stream) {
+  cfg_ddim_kernel<<<grid_for(static_cast<long long>(K) * n_item, 256), 256, 0, stream>>>(
+      x, eps2, K, n_item, guidance, sqrtf(a_t), sqrtf(1.f - a_t), sqrtf(a_prev), sqrtf(1.f - a_prev), x_inv, items, fhw);
+  FZ_CUDA(cudaGetLastError());
+  return FZ_OK;
+}
+
 extern "C" int fz_cfg_ddim_step(float* x, const float* eps2, long long n, float guidance, float a_t, float a_prev, const float* x_inv,
                                 const float* mask_a, const float* mask_b, long long fhw, int apply_blend, cudaStream_t stream) {
   FZ_CHECK_ARG(x && eps2, "fz_cfg_ddim_step: null pointer");
   FZ_CHECK_ARG(!apply_blend || (x_inv && mask_a && fhw > 0), "fz_cfg_ddim_step: blend needs x_inv and mask");
-  cfg_ddim_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, eps2, n, guidance, sqrtf(a_t), sqrtf(1.f - a_t), sqrtf(a_prev), sqrtf(1.f - a_prev),
-                                                        x_inv, mask_a, mask_b, fhw, apply_blend);
-  FZ_CUDA(cudaGetLastError());
-  return FZ_OK;
+  CfgItems items;
+  memset(&items, 0, sizeof(items));
+  items.mask_a[0] = mask_a;
+  items.mask_b[0] = mask_b;
+  items.apply_blend[0] = apply_blend;
+  return cfg_ddim_launch(x, eps2, 1, n, guidance, a_t, a_prev, x_inv, items, fhw, stream);
+}
+
+extern "C" int fz_cfg_ddim_step_batched(float* x, const float* eps2, int K, long long n_item, float guidance, float a_t, float a_prev,
+                                        const float* x_inv, const float* const* mask_a, const float* const* mask_b, const int* apply_blend,
+                                        long long fhw, cudaStream_t stream) {
+  FZ_CHECK_ARG(x && eps2 && n_item > 0, "fz_cfg_ddim_step_batched: null pointer");
+  FZ_CHECK_ARG(K >= 1 && K <= kCfgMaxItems, "fz_cfg_ddim_step_batched: K=%d unsupported (1..%d)", K, kCfgMaxItems);
+  CfgItems items;
+  memset(&items, 0, sizeof(items));
+  for (int k = 0; k < K; ++k) {
+    items.mask_a[k] = mask_a ? mask_a[k] : nullptr;
+    items.mask_b[k] = mask_b ? mask_b[k] : nullptr;
+    items.apply_blend[k] = apply_blend ? apply_blend[k] : 0;
+    FZ_CHECK_ARG(!items.apply_blend[k] || (x_inv && items.mask_a[k] && fhw > 0), "fz_cfg_ddim_step_batched: item %d: blend needs x_inv and mask", k);
+  }
+  return cfg_ddim_launch(x, eps2, K, n_item, guidance, a_t, a_prev, x_inv, items, fhw, stream);
 }
 
 extern "C" int fz_blend_mask(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int r, int ldm, int ntok, const float* word_w,

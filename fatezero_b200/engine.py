@@ -68,6 +68,9 @@ class UNetEngine:
         self._text_kv: Dict[str, tuple] = {}
         self._foreign = None  # reference-protocol controller of the current forward (slow path), see _foreign_attention
         self.shard = None  # frame sharding over GPUs: (rank, world, process group), see set_frame_shard
+        # batched edit of K prompts (controller.prompt_groups = K > 1): the GroupNorm chunking is planned per prompt (NB / K images) so
+        # that every prompt's statistics are bitwise those of its own single-prompt pass; None = planned for the whole batch
+        self._images_per_item = None
         self._prepare({k: v.detach() for k, v in unet.state_dict().items()})
 
     # ---------------------------------------------------------------------------------------------------------------
@@ -99,7 +102,7 @@ class UNetEngine:
         every rank pushes its per-image (sum, sumsq) [NB, G] into each peer's inbox (512 B .. 2 KiB over NVLink), fz_gn_combine waits for the
         peers and folds everything into the layout the apply kernel reads."""
         if self.shard is None:
-            return ops.groupnorm(x3, gamma, beta, eps, self.groups, F, silu)
+            return ops.groupnorm(x3, gamma, beta, eps, self.groups, F, silu, images_per_item=self._images_per_item)
         rank, world, _ = self.shard
         ar = self.arena
         NB, G = x3.shape[0], self.groups
@@ -373,7 +376,8 @@ class UNetEngine:
         scale = d ** -0.5
         bp = p + ".transformer_blocks.0"
         xr = x.view(M, C)
-        n = ops.groupnorm(x.view(NB, S, C), w[p + ".norm.weight"], w[p + ".norm.bias"], 1e-6, self.groups, 1, False)
+        n = ops.groupnorm(x.view(NB, S, C), w[p + ".norm.weight"], w[p + ".norm.bias"], 1e-6, self.groups, 1, False,
+                          images_per_item=self._images_per_item)
         h = ops.gemm(n.view(M, C), w[p + ".proj_in.weight"], bias=w[p + ".proj_in.bias"])
         # ---- attn1: sparse-causal spatio-temporal self-attention (attention_register.py:131-218)
         if "SparseCausalAttention_index" in self.mc:
@@ -483,6 +487,12 @@ class UNetEngine:
         if text.shape[0] != B:
             raise ValueError(f"encoder_hidden_states batch {text.shape[0]} != sample batch {B}")
         self._ensure_text(text)
+        groups = getattr(ctrl, "prompt_groups", 1) if ctrl is not None else 1
+        if groups > 1 and self.shard is not None:
+            raise NotImplementedError("a batched multi-prompt edit does not run frame-sharded")
+        if groups > 1 and B % groups:
+            raise ValueError(f"batch {B} does not split into {groups} prompt groups")
+        self._images_per_item = NB // groups if groups > 1 else None
         if ctrl is not None:
             ctrl.begin_forward(B, F)
         temb_all = self.time_embedding(t)

@@ -140,16 +140,22 @@ def _workspace(device, nbytes: int) -> torch.Tensor:
 
 
 def groupnorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, groups: int, frames_per_stat: int, silu: bool,
-              out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """x [NB, HW, C] fp16; statistics over (C/groups, HW, frames_per_stat consecutive NB rows)."""
+              out: Optional[torch.Tensor] = None, images_per_item: Optional[int] = None) -> torch.Tensor:
+    """x [NB, HW, C] fp16; statistics over (C/groups, HW, frames_per_stat consecutive NB rows).
+    images_per_item (batched edits): x holds NB / images_per_item items (prompts); each image's statistics are then bitwise those of a
+    call over its item alone."""
     _chk(x, f16, "groupnorm")
     NB, HW, Cc = x.shape
     assert x.is_contiguous()
     if out is None:
         out = torch.empty_like(x)
     ws = _workspace(x.device, 1 << 20)  # per-(image, chunk, group) partial sums
-    _lib.call("fz_groupnorm_nhwc_f16", _p(x), _p(out), NB, HW, Cc, groups, frames_per_stat, _p(gamma), _p(beta), float(eps), int(silu),
-              _p(ws), _stream())
+    if images_per_item is None:
+        _lib.call("fz_groupnorm_nhwc_f16", _p(x), _p(out), NB, HW, Cc, groups, frames_per_stat, _p(gamma), _p(beta), float(eps), int(silu),
+                  _p(ws), _stream())
+    else:
+        _lib.call("fz_groupnorm_batched_nhwc_f16", _p(x), _p(out), NB, HW, Cc, groups, frames_per_stat, int(images_per_item), _p(gamma),
+                  _p(beta), float(eps), int(silu), _p(ws), _stream())
     return out
 
 
@@ -250,6 +256,21 @@ def cfg_ddim_step(x: torch.Tensor, eps2: torch.Tensor, guidance: float, a_t: flo
               fhw, int(apply_blend), _stream())
 
 
+def cfg_ddim_step_batched(x: torch.Tensor, eps2: torch.Tensor, guidance: float, a_t: float, a_prev: float, x_inv=None,
+                          blends: Optional[Sequence[Optional[dict]]] = None):
+    """x [K, 4, F, h, w] fp32 (K prompts), eps2 [2K, ...] = [uncond_1..K ; cond_1..K]; blends: one latent_blend_args() dict (or None) per
+    item, all sharing x_inv."""
+    K = x.shape[0]
+    fhw = x.shape[-3] * x.shape[-2] * x.shape[-1]
+    blends = list(blends) if blends is not None else [None] * K
+    assert len(blends) == K and eps2.shape[0] == 2 * K
+    ma = (C.c_void_p * K)(*[None if b is None else b["mask_a"].data_ptr() for b in blends])
+    mb = (C.c_void_p * K)(*[None if b is None or b["mask_b"] is None else b["mask_b"].data_ptr() for b in blends])
+    ap = (C.c_int * K)(*[int(b is not None and bool(b["apply_blend"])) for b in blends])
+    _lib.call("fz_cfg_ddim_step_batched", _p(x), _p(eps2), K, x.numel() // K, float(guidance), float(a_t), float(a_prev), _p(x_inv), ma, mb, ap,
+              fhw, _stream())
+
+
 def blend_mask(maps: Sequence[torch.Tensor], word_w: torch.Tensor, th: float, h: int, w: int) -> torch.Tensor:
     """maps: list of [F, heads, r*r, ld] (fp16 cache slabs or fp16 running sums) -> mask [F, h, w] float 0/1."""
     m0 = maps[0]
@@ -302,8 +323,10 @@ def cross_heatmaps(maps: Sequence[torch.Tensor], ntok: int) -> torch.Tensor:
 def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, out: torch.Tensor, *, S_q: int, keys_per_slot: int, n_src: int, d: int,
               heads: int, F: int, BF: int, scale: float, src_index: Sequence[Sequence[int]], edit_bf_start: int = 0,
               row_mode: int = _lib.ATTN_NONE, store=None, base=None, cache_ld: int = 0, acc=None, xedit=None, mask=None, dbg=None,
-              causal: bool = False):
-    """q/k: strided 2-D views (rows, ld) whose column h*d starts head h; vt [n_src, heads, d, vt_ld]; out [BF*S_q, ldo]."""
+              causal: bool = False, groups: Optional[Sequence[dict]] = None):
+    """q/k: strided 2-D views (rows, ld) whose column h*d starts head h; vt [n_src, heads, d, vt_ld]; out [BF*S_q, ldo].
+    groups (batched edits): one dict(row_mode=, mask=, acc=, xedit=) per edited row group of F rows after edit_bf_start, all reading `base`;
+    row_mode / acc / xedit / mask must then be left at their defaults."""
     a = AttnArgs()
     a.q, a.ldq = _p(q), q.stride(0)
     a.k, a.ldk = _p(k), k.stride(0)
@@ -321,5 +344,19 @@ def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, out: torch.Ten
     a.xedit, a.mask = _p(xedit), _p(mask)
     a.dbg = _p(dbg)
     a.causal = int(causal)
-    _lib.call("fz_attention_f16", C.byref(a), _stream())
+    if groups is None:
+        _lib.call("fz_attention_f16", C.byref(a), _stream())
+        return out
+    if row_mode != _lib.ATTN_NONE or acc is not None or xedit is not None or mask is not None:
+        raise ValueError("fatezero_b200.ops.attention: with groups=, the hook arguments belong to the groups")
+    if not 1 <= len(groups) <= _lib.MAX_ATTN_GROUPS:
+        raise ValueError(f"fatezero_b200.ops.attention: {len(groups)} groups (1..{_lib.MAX_ATTN_GROUPS})")
+    gs = _lib.AttnGroups()
+    gs.n_groups = len(groups)
+    for i, g in enumerate(groups):
+        gs.g[i].row_mode = int(g.get("row_mode", _lib.ATTN_NONE))
+        gs.g[i].xedit, gs.g[i].mask, gs.g[i].acc = _p(g.get("xedit")), _p(g.get("mask")), _p(g.get("acc"))
+        if g.get("acc") is not None:
+            a.acc_ld = g["acc"].stride(2)
+    _lib.call("fz_attention_grouped_f16", C.byref(a), C.byref(gs), _stream())
     return out

@@ -375,13 +375,13 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         return self.scheduler.timesteps[t_start:], num_inference_steps - t_start
 
     # ---- edit -----------------------------------------------------------------------------------------------------------
-    def p2preplace_edit(self, **kwargs):
-        """p2p_ddim_spatial_temporal.py:172-222."""
-        len_source = len(kwargs["source_prompt"].split(" "))
-        len_target = len(kwargs["prompt"].split(" "))
+    def _make_edit_controller(self, prompt: str, source_prompt: str, num_inference_steps: int, **kwargs):
+        """The make_controller call of p2p_ddim_spatial_temporal.py:176-193: one target prompt against the inversion store."""
+        len_source = len(source_prompt.split(" "))
+        len_target = len(prompt.split(" "))
         equal_length = len_source == len_target
-        edit_controller = attention_util.make_controller(
-            self.tokenizer, [kwargs["source_prompt"], kwargs["prompt"]], NUM_DDIM_STEPS=kwargs["num_inference_steps"],
+        return attention_util.make_controller(
+            self.tokenizer, [source_prompt, prompt], NUM_DDIM_STEPS=num_inference_steps,
             is_replace_controller=kwargs.get("is_replace_controller", True) and equal_length,
             cross_replace_steps=kwargs["cross_replace_steps"], self_replace_steps=kwargs["self_replace_steps"],
             blend_words=kwargs.get("blend_words", None), equilizer_params=kwargs.get("eq_params", None),
@@ -389,6 +389,10 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
             blend_th=kwargs.get("blend_th", (0.3, 0.3)), blend_self_attention=kwargs.get("blend_self_attention", None),
             blend_latents=kwargs.get("blend_latents", None), save_path=kwargs.get("save_path", None),
             save_self_attention=kwargs.get("save_self_attention", True), disk_store=kwargs.get("disk_store", False))
+
+    def p2preplace_edit(self, **kwargs):
+        """p2p_ddim_spatial_temporal.py:172-222."""
+        edit_controller = self._make_edit_controller(**kwargs)
         attention_util.register_attention_control(self, edit_controller)
         sdimage_output = self.sd_ddim_pipeline(controller=edit_controller, **kwargs)
         mask_list = edit_controller.latent_blend.mask_list if hasattr(edit_controller.latent_blend, "mask_list") else None
@@ -399,6 +403,72 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         self.last_edit_controller = edit_controller
         attention_util.register_attention_control(self, self.empty_controller)
         return {"sdimage_output": sdimage_output, "attention_output": attention_output, "mask_list": mask_list}
+
+    MAX_BATCH_ROWS = 128  # CFG rows (2 x prompts x frames) of one grouped attention launch
+
+    @torch.no_grad()
+    def p2preplace_edit_batch(self, prompts: List[str], p2p_configs: List[dict], source_prompt: str, latents: torch.Tensor,
+                              num_inference_steps: int, guidance_scale: float, save_path: Optional[str] = None, output_type: str = "pil",
+                              negative_prompt=None, callback=None, callback_steps: int = 1):
+        """Edit ONE inverted clip (`latents`: x_T [1, 4, F, h, w] of the inversion held by `self.store_controller`) with several target
+        prompts in one batched pass: every UNet forward runs the K prompts' CFG rows together.  Prompt k gets, bit for bit, what
+        `p2preplace_edit(prompt=prompts[k], **p2p_configs[k], ...)` gives it (latents, masks, running attention sums).  Returns one
+        p2preplace_edit result dict per prompt; `self.last_edit_controllers` holds the K edit controllers.  callback(i, t, latents[K, ...])."""
+        prompts = list(prompts)
+        p2p_configs = [dict(c) for c in p2p_configs]
+        K = len(prompts)
+        if K == 0 or len(p2p_configs) != K:
+            raise ValueError(f"p2preplace_edit_batch: {K} prompts and {len(p2p_configs)} p2p configs")
+        if K > attention_util._lib.MAX_ATTN_GROUPS:
+            raise ValueError(f"p2preplace_edit_batch: at most {attention_util._lib.MAX_ATTN_GROUPS} prompts per batch, got {K}")
+        if latents is None or latents.dim() != 5 or latents.shape[0] != 1:
+            raise ValueError("p2preplace_edit_batch: latents must be the inverted clip's x_T of shape [1, 4, F, h, w]")
+        F = latents.shape[2]
+        if 2 * K * F > self.MAX_BATCH_ROWS:
+            raise ValueError(f"p2preplace_edit_batch: 2 x {K} prompts x {F} frames = {2 * K * F} CFG rows exceed {self.MAX_BATCH_ROWS}")
+        for k, c in enumerate(p2p_configs):
+            if int(c.get("num_inference_steps", num_inference_steps)) != int(num_inference_steps):
+                raise ValueError(f"p2preplace_edit_batch: prompt {k} asks for num_inference_steps={c['num_inference_steps']}")
+            if float(c.get("guidance_scale", guidance_scale)) != float(guidance_scale):
+                raise ValueError(f"p2preplace_edit_batch: prompt {k} asks for guidance_scale={c['guidance_scale']}")
+            if float(c.get("eta", 0.0)) != 0.0:
+                raise NotImplementedError("FateZero's DDIM path is deterministic (eta = 0)")
+        engine = getattr(self.unet, "_engine", None)  # not built here: nothing below may touch the GPU before the checks pass
+        if getattr(engine, "shard", None) is not None:
+            raise NotImplementedError("p2preplace_edit_batch: frame-sharded batched edits are not supported")
+        store = self.store_controller
+        if getattr(store, "disk_store", False) or getattr(store, "host_spill", False):
+            raise NotImplementedError("p2preplace_edit_batch: disk_store / host_spill inversion stores are edited one prompt at a time")
+        drop = ("prompt", "source_prompt", "num_inference_steps", "guidance_scale", "eta", "save_path", "latents", "output_type",
+                "negative_prompt", "callback", "callback_steps")
+        edits = [self._make_edit_controller(prompt=pr, source_prompt=source_prompt, num_inference_steps=num_inference_steps, save_path=save_path,
+                                            **{k: v for k, v in c.items() if k not in drop})
+                 for pr, c in zip(prompts, p2p_configs)]
+        batch = attention_util.AttentionControlEditBatch(edits)
+        attention_util.register_attention_control(self, batch)
+        try:
+            out = self.sd_ddim_pipeline(prompt=prompts, num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
+                                        negative_prompt=negative_prompt, latents=latents, output_type="latent", callback=callback,
+                                        callback_steps=callback_steps, controller=batch)
+        finally:
+            attention_util.register_attention_control(self, self.empty_controller)
+        lat = out.images
+        results = []
+        for k, (pr, e) in enumerate(zip(prompts, edits)):
+            lk = lat[k:k + 1]
+            if output_type == "latent":
+                sd = StableDiffusionPipelineOutput(images=lk, nsfw_content_detected=None)
+            else:
+                image = self.decode_latents(lk)  # per prompt: the VAE's GroupNorm chunking depends on the batch
+                sd = StableDiffusionPipelineOutput(images=self.numpy_to_pil(image) if output_type == "pil" else image, nsfw_content_detected=None)
+            mask_list = e.latent_blend.mask_list if hasattr(e.latent_blend, "mask_list") else None
+            attention_output = None
+            if len(e.attention_store.keys()) > 0 and output_type != "latent":
+                from .visualization import show_cross_attention
+                attention_output = show_cross_attention(self.tokenizer, pr, e, 16, ["up", "down"])
+            results.append({"sdimage_output": sd, "attention_output": attention_output, "mask_list": mask_list})
+        self.last_edit_controllers = edits
+        return results
 
     @torch.no_grad()
     def __call__(self, **kwargs):
@@ -435,7 +505,19 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         do_cfg = guidance_scale > 1.0
         if not do_cfg:
             raise NotImplementedError("guidance_scale <= 1 (no CFG batch) is not an editing configuration of the reference YAMLs")
-        text_embeddings = self._encode_prompt(prompt, device, num_images_per_prompt, do_cfg, negative_prompt).to(self.unet.device)
+        is_batch = isinstance(controller, attention_util.AttentionControlEditBatch)
+        if is_batch:
+            # K prompts of one clip: [uncond_1..K ; cond_1..K], each prompt encoded on its own so that its embedding is bitwise the one of
+            # its single-prompt pass
+            if num_images_per_prompt != 1 or latents is None or len(prompt) != controller.prompt_groups:
+                raise ValueError("a batched edit needs one prompt per edit controller, num_images_per_prompt=1 and the inverted latents")
+            negs = negative_prompt if isinstance(negative_prompt, list) else [negative_prompt] * len(prompt)
+            per = [self._encode_prompt(pr, device, 1, do_cfg, ng).to(self.unet.device) for pr, ng in zip(prompt, negs)]
+            text_embeddings = torch.cat([e[:1] for e in per] + [e[1:] for e in per])
+            if latents.shape[0] == 1:
+                latents = latents.expand(len(prompt), *latents.shape[1:])
+        else:
+            text_embeddings = self._encode_prompt(prompt, device, num_images_per_prompt, do_cfg, negative_prompt).to(self.unet.device)
         self.scheduler.set_timesteps(num_inference_steps, device=device)
         timesteps = [int(t) for t in self.scheduler.timesteps]
         if latents is None:
@@ -451,7 +533,7 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         latents_dtype = latents.dtype
         dev = self.unet.device
         text_embeddings = text_embeddings.contiguous()
-        is_edit = isinstance(controller, attention_util.AttentionControlEdit)
+        is_edit = is_batch or isinstance(controller, attention_util.AttentionControlEdit)
         step = self.scheduler.config.num_train_timesteps // self.scheduler.num_inference_steps
         n = len(timesteps)
 
@@ -461,7 +543,13 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
             eps2 = self.unet(x2, t, encoder_hidden_states=text).sample
             blend = ctrl.latent_blend_args(x.shape[-2], x.shape[-1]) if is_edit else None
             a_t, a_prev = self._alpha(t), self._alpha(t - step)
-            if blend is not None:
+            if is_batch:
+                live = [b for b in blend if b is not None]
+                x_inv = live[0]["x_inv"].contiguous() if live else None
+                if any(b["x_inv"].data_ptr() != live[0]["x_inv"].data_ptr() for b in live[1:]):
+                    raise RuntimeError("the edits of a batch disagree on the inverted latent of this step")
+                ops.cfg_ddim_step_batched(x, eps2.contiguous(), guidance_scale, a_t, a_prev, x_inv=x_inv, blends=blend)
+            elif blend is not None:
                 ops.cfg_ddim_step(x, eps2.contiguous(), guidance_scale, a_t, a_prev, x_inv=blend["x_inv"].contiguous(),
                                   mask_a=blend["mask_a"], mask_b=blend["mask_b"], apply_blend=blend["apply_blend"])
             else:

@@ -113,6 +113,26 @@ typedef struct fz_attn_args {
 
 int fz_attention_f16(const fz_attn_args_t* args, fz_stream_t stream);
 
+/* Several edited row groups in one launch: one inverted clip edited with n_groups target prompts under one CFG batch
+ * [uncond_1..K ; cond_1..K].  Rows bf >= args->edit_bf_start belong to group g = (bf - edit_bf_start) / F and read cache frame
+ * fc = (bf - edit_bf_start) % F of the SAME `base` slab [F, heads, S_q, cache_ld] (the inversion map of the step); BF - edit_bf_start
+ * must equal n_groups * F.  The per-row hook fields of `args` (row_mode, xedit, mask, acc) are ignored: each group brings its own.
+ * Modes NONE / REPLACE / BLEND / CROSSEDIT may be mixed in one launch; STORE is refused.  BF <= 128 (fz_attention_f16: BF <= 64).
+ * Every row computes exactly what fz_attention_f16 computes for it with its group's hook, so each group's rows and `acc` are bitwise
+ * equal to a launch over that group alone. */
+#define FZ_ATTN_MAX_GROUPS 8
+typedef struct fz_attn_group {
+  int row_mode;                     /* FZ_ATTN_NONE / REPLACE / BLEND / CROSSEDIT                                       */
+  const float* xedit;               /* CROSSEDIT: device table (layout above)                                           */
+  const float* mask;                /* BLEND: device [F, S_q], 1 = keep current row                                     */
+  void* acc;                        /* fp16 running sum slab [F, heads, S_q, args->acc_ld] or NULL                       */
+} fz_attn_group_t;
+typedef struct fz_attn_groups {
+  int n_groups;                     /* 1 .. FZ_ATTN_MAX_GROUPS                                                          */
+  fz_attn_group_t g[FZ_ATTN_MAX_GROUPS];
+} fz_attn_groups_t;
+int fz_attention_grouped_f16(const fz_attn_args_t* args, const fz_attn_groups_t* groups, fz_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * HBM-bound kernels of the step
  * --------------------------------------------------------------------------------------------------------- */
@@ -121,6 +141,11 @@ int fz_attention_f16(const fz_attn_args_t* args, fz_stream_t stream);
  * zero-filled once before the first call and is left consistent by every call (calls sharing it must be stream-ordered). */
 int fz_groupnorm_nhwc_f16(const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, const float* gamma,
                           const float* beta, float eps, int silu, void* workspace_f64, fz_stream_t stream);
+/* Same normalisation of a batch made of NB / images_per_item items (prompts of a batched edit): the partial-sum chunking of the
+ * statistics pass is planned for images_per_item images, so every image's statistics are bitwise those of a call over its item alone
+ * (fz_groupnorm_nhwc_f16 plans it for NB images).  images_per_item must divide NB and be a multiple of frames_per_stat. */
+int fz_groupnorm_batched_nhwc_f16(const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, int images_per_item,
+                                  const float* gamma, const float* beta, float eps, int silu, void* workspace_f64, fz_stream_t stream);
 
 /* Frame-sharded GroupNorm (one clip's frames over several GPUs, SURVEY.md 8(e); resnet.py:338,369 normalise over ALL frames):
  * fz_groupnorm_stats_f16 leaves float2 (sum, sumsq) [NB][groups] at workspace_f64 + 768 KiB; the caller all-reduces the per-set sums over
@@ -150,6 +175,12 @@ int fz_ddim_invert_step(float* x, const float* eps, long long n, float alpha_pre
 /* x <- CFG + DDIM eta=0 step (+ latent blend x_inv + m (x - x_inv)) (p2p_ddim_spatial_temporal.py:400-407; spatial_blend.py:116-122) */
 int fz_cfg_ddim_step(float* x, const float* eps2, long long n, float guidance, float alpha_t, float alpha_prev, const float* x_inv,
                      const float* mask_a, const float* mask_b, long long fhw, int apply_blend, fz_stream_t stream);
+/* The same step for K <= 8 items (prompts of a batched edit): x [K, n_item], eps2 [uncond_1..K ; cond_1..K] x n_item, x_inv [n_item]
+ * shared by every item; mask_a / mask_b / apply_blend: HOST arrays [K] (device mask pointers, NULL where an item does not blend).
+ * Item k gets exactly the arithmetic of fz_cfg_ddim_step on its slice (which is this call with K = 1). */
+int fz_cfg_ddim_step_batched(float* x, const float* eps2, int K, long long n_item, float guidance, float alpha_t, float alpha_prev,
+                             const float* x_inv, const float* const* mask_a, const float* const* mask_b, const int* apply_blend,
+                             long long fhw, fz_stream_t stream);
 /* blend mask from cached cross maps (spatial_blend.py:24-39,78-111); maps: HOST array of device pointers, word_w: HOST [ntok] */
 int fz_blend_mask(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int r, int ldm, int ntok, const float* word_w,
                   float th, int h, int w, float* out, fz_stream_t stream);
