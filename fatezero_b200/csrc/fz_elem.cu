@@ -167,7 +167,9 @@ __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(const __half* __re
   const int tx = threadIdx.x % TX, ty = threadIdx.x / TX;
   const int TY = kGnThreads / TX;
   if (ty >= TY) return;
-  float sc[SLOTS][8], sh[SLOTS][8];
+  // y = (x - mean) * (rstd * gamma) + beta: centring first keeps a (near-)constant group exact; a fused shift beta - mean * rstd * gamma
+  // would carry a rounding error of 2^-24 |mean| rstd |gamma| into every output
+  float sc[SLOTS][8], mn[SLOTS][8], sh[SLOTS][8];
 #pragma unroll
   for (int s = 0; s < SLOTS; ++s) {
     const int cv = tx + s * TX;
@@ -179,7 +181,8 @@ __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(const __half* __re
     for (int e = 0; e < 8; ++e) {
       const int g = (cv * 8 + e) / cpg;
       sc[s][e] = s_rstd[g] * gg[e];
-      sh[s][e] = bb[e] - s_mean[g] * s_rstd[g] * gg[e];
+      mn[s][e] = s_mean[g];
+      sh[s][e] = bb[e];
     }
   }
   const int p0 = blockIdx.x * px_per_cta;
@@ -205,7 +208,7 @@ __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(const __half* __re
           Half8 o;
 #pragma unroll
           for (int e = 0; e < 8; ++e) {
-            float v = fmaf(__half2float(h[u][s].v[e]), sc[s][e], sh[s][e]);
+            float v = fmaf(__half2float(h[u][s].v[e]) - mn[s][e], sc[s][e], sh[s][e]);
             if (silu) v = __fdividef(v, 1.0f + __expf(-v));  // fast reciprocal: the IEEE division made this kernel MUFU/issue-bound
             o.v[e] = __float2half_rn(v);
           }
@@ -259,7 +262,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
     }
   }
   float v[ROWS][NV][8];
-  float sum[ROWS], sq[ROWS];
+  float sum[ROWS], mean[ROWS], sq[ROWS];
 #pragma unroll
   for (int r = 0; r < ROWS; ++r) {
     sum[r] = 0.f;
@@ -279,16 +282,22 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
     for (int o = 16; o > 0; o >>= 1) sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], o);
   }
   const float inv_c = 1.0f / C;
+  // the mean sum / C, rounded as a division rounds it (one fma correction of sum * (1/C); a division's slow path would cost this kernel a
+  // stack frame): exact for a constant row, whose sum of fp16 values is exact in fp32
 #pragma unroll
   for (int r = 0; r < ROWS; ++r) {
-    const float mean = sum[r] * inv_c;
+    const float q = sum[r] * inv_c;
+    mean[r] = fmaf(fmaf(-q, static_cast<float>(C), sum[r]), inv_c, q);
+  }
+#pragma unroll
+  for (int r = 0; r < ROWS; ++r) {
     sq[r] = 0.f;
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
       if (lane + i * 32 < CV) {
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          const float d = v[r][i][e] - mean;
+          const float d = v[r][i][e] - mean[r];
           sq[r] = fmaf(d, d, sq[r]);
         }
       }
@@ -309,13 +318,14 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
         const long long row = row0 + r;
         if (row < M) {
           const float rstd = rsqrtf(sq[r] * inv_c + eps);
-          const float shift = -sum[r] * inv_c * rstd;  // (x - mean) * rstd == x * rstd + shift
+          // from the centred value: a fused x * rstd + (-mean * rstd) rounds the shift, an absolute error of 2^-24 |mean| rstd that
+          // swamps beta on a (near-)constant row, where rstd approaches eps^-1/2
           Half8 o;
           __half2* o2 = reinterpret_cast<__half2*>(&o);
 #pragma unroll
           for (int e = 0; e < 4; ++e)
-            o2[e] = __floats2half2_rn(fmaf(fmaf(v[r][i][2 * e], rstd, shift), gg[2 * e], bb[2 * e]),
-                                      fmaf(fmaf(v[r][i][2 * e + 1], rstd, shift), gg[2 * e + 1], bb[2 * e + 1]));
+            o2[e] = __floats2half2_rn(fmaf((v[r][i][2 * e] - mean[r]) * rstd, gg[2 * e], bb[2 * e]),
+                                      fmaf((v[r][i][2 * e + 1] - mean[r]) * rstd, gg[2 * e + 1], bb[2 * e + 1]));
           *reinterpret_cast<Half8*>(y + row * C + cv * 8) = o;
         }
       }
@@ -735,11 +745,14 @@ __global__ void __launch_bounds__(256) blend_mask_kernel(const __grid_constant__
     pooled[px] = m;
   }
   __syncthreads();
+  // F.interpolate(mode="nearest") source index: min(floor(dst * (float)in / out), in - 1) in fp32 (the exact integer quotient
+  // (dst * in) / out differs for some sizes, e.g. in = 16, out = 82)
+  const float sy_scale = static_cast<float>(p.r) / p.h, sx_scale = static_cast<float>(p.r) / p.w_out;
   // max over the RESIZED grid == max over the source pixels that the nearest resize actually samples
   float lm = 0.f;
   for (int i = threadIdx.x; i < p.h * p.w_out; i += blockDim.x) {
     const int y = i / p.w_out, x = i % p.w_out;
-    const int sy = min(p.r - 1, (y * p.r) / p.h), sx = min(p.r - 1, (x * p.r) / p.w_out);
+    const int sy = min(p.r - 1, static_cast<int>(floorf(y * sy_scale))), sx = min(p.r - 1, static_cast<int>(floorf(x * sx_scale)));
     lm = fmaxf(lm, pooled[sy * p.r + sx]);
   }
   atomicMax(reinterpret_cast<int*>(&s_max), __float_as_int(fmaxf(lm, 0.f)));
@@ -747,7 +760,7 @@ __global__ void __launch_bounds__(256) blend_mask_kernel(const __grid_constant__
   const float mx = s_max;
   for (int i = threadIdx.x; i < p.h * p.w_out; i += blockDim.x) {
     const int y = i / p.w_out, x = i % p.w_out;
-    const int sy = min(p.r - 1, (y * p.r) / p.h), sx = min(p.r - 1, (x * p.r) / p.w_out);
+    const int sy = min(p.r - 1, static_cast<int>(floorf(y * sy_scale))), sx = min(p.r - 1, static_cast<int>(floorf(x * sx_scale)));
     const float v = pooled[sy * p.r + sx];
     // reference: (v / mx) > th, with 0/0 = NaN -> False
     p.out[(static_cast<long long>(f) * p.h + y) * p.w_out + x] = (mx > 0.f && (v / mx) > p.th) ? 1.f : 0.f;
@@ -1060,7 +1073,8 @@ __global__ void __launch_bounds__(256) cross_heatmap_kernel(const __grid_constan
   for (int w = 1; w < (blockDim.x >> 5); ++w) vmax = fmaxf(vmax, s_max[w]);
   nv = 0;
   for (int px = threadIdx.x; px < p.rr; px += blockDim.x, ++nv)
-    p.out[(static_cast<long long>(f) * p.ntok + tok) * p.rr + px] = static_cast<unsigned char>(fminf(255.f, 255.f * vals[nv] / vmax));
+    p.out[(static_cast<long long>(f) * p.ntok + tok) * p.rr + px] =
+        vmax > 0.f ? static_cast<unsigned char>(fminf(255.f, 255.f * vals[nv] / vmax)) : 0;  // all-zero column: 0, not 0/0
 }
 
 }  // namespace fz

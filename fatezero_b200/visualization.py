@@ -79,7 +79,9 @@ def show_cross_attention(tokenizer, prompts, attention_store, res: int, from_whe
         tiles = []
         for i, tok in enumerate(tokens):
             heat = frame[:, :, i]
-            heat = heat.numpy() if heat.dtype == torch.uint8 else (255 * heat / heat.max()).clamp(0, 255).numpy().astype(np.uint8)
+            if heat.dtype != torch.uint8:  # an all-zero map is black (0/0 would be NaN, whose uint8 cast is undefined)
+                heat = (255 * heat / heat.max()).nan_to_num(0.0).clamp(0, 255)
+            heat = heat.numpy().astype(np.uint8)
             tile = np.array(Image.fromarray(np.repeat(heat[:, :, None], 3, axis=2)).resize((256, 256)))
             tiles.append(_caption(tile, tokenizer.decode(int(tok))))
         strips.append(np.concatenate(tiles, axis=1))

@@ -17,6 +17,21 @@ Attention outputs (P rounded to fp16 before PV, fp32 accumulation) pass when
 
   the middle term covers P entries in the fp16 subnormal range, whose rounding error is absolute (<= 2^-25), not relative; the kernels
   divide by a row sum >= 1, so it is not amplified.
+
+GroupNorm / LayerNorm outputs (test_gpu_elem_edges.py): y = gamma (x - mu) rstd + beta, rstd = 1 / sqrt(var + eps), mu and var the fp64
+statistics of the fp16 inputs, pass when
+
+    |got - y| <= ulp16(y) + gamma rstd |mu - fp32(mu)| + c * 2^-24 * (|gamma| rstd sqrt(n_stat) (|x - mu| + sigma) + |beta|)
+
+  the second term is the rounding of the mean to fp32, which no fp32 kernel can avoid; it is 0 when the mean is representable (a
+  constant row).  The third is a Welford-class statistics error: it scales with sigma, never with |mu|, so a kernel that loses the
+  variance to cancellation (E[x^2] - mu^2) or rounds a fused shift -mu * rstd fails it.  With SiLU the pre-activation terms are
+  multiplied by max|silu'| = 1.1 and (5 + 1.2 |y|) 2^-23 |silu(y)| is added for __expf and __fdividef.
+  The GroupNorm statistics ARE E[x^2] - mu^2 from fp32 partial sums (DESIGN.md, known limits); groups far from zero mean are therefore
+  checked against that bound plus  c_dc * 2^-24 * |gamma| (mu / sigma_eps)^2 (1 + |x - mu| rstd),  sigma_eps = sqrt(var + eps).
+
+Element-wise fp32 steps (DDIM, CFG + DDIM + blend, out_temporal, the time embedding): |got - ref64| <= c * 2^-24 * sum|terms|, the
+terms being the expression evaluated on absolute values (the running-error bound of its fp32 evaluation).
 """
 import math
 
@@ -144,3 +159,235 @@ def check_probs(got, p, report=None, key="", k_ulp: float = 1.0) -> dict:
     """Stored probabilities: within k_ulp fp16 ulps of fp16(softmax64)."""
     r = p.double().half().double()
     return check_bound(got, r, k_ulp * ulp16(r), report, key)
+
+
+# ---------------------------------------------------------------------------------------------------------------- normalisation
+# c of the norm bound and c_dc of the GroupNorm DC-offset term.  Measured on an H100 SXM 80 GB (132 SMs, 700 W power limit) over every
+# norm case of test_gpu_elem_edges.py (each records its own c_needed / c_dc_needed in the report): the largest c a strict case needed was
+# 0.14 (GroupNorm at mean/sigma = 64), the largest c_dc 0.28 (near-constant groups).
+C_NORM = 0.5
+C_DC = 1.0
+
+
+def f32(x: float) -> float:
+    """The value a kernel sees for a float argument (passed as a C float)."""
+    return torch.tensor(x, dtype=torch.float32).item()
+
+
+def norm_check(got, x64, dims, gamma, beta, eps: float, silu=False, report=None, key="", c: float = C_NORM, c_dc=None) -> dict:
+    """got and x64 of one shape; statistics over `dims` of x64; gamma / beta fp64, broadcastable to x64.  Bound: see the module docstring
+    (c_dc None: the strict bound; otherwise the strict bound plus the DC-offset term, and the strict ratio is only recorded)."""
+    n = math.prod(x64.shape[d] for d in dims)
+    mu = x64.mean(dims, keepdim=True)
+    d = x64 - mu
+    var = (d * d).mean(dims, keepdim=True)
+    rstd = (var + f32(eps)).rsqrt()
+    g, b = gamma.double(), beta.double()
+    out = d * rstd * g + b
+    ga = g.abs()
+    acc = U32 * (ga * rstd * math.sqrt(n) * (d.abs() + var.sqrt()) + b.abs())
+    fixed = ga * rstd * (mu - mu.float().double()).abs()
+    dc = U32 * ga * (mu * rstd) ** 2 * (1 + d.abs() * rstd)
+    if silu:
+        y = out
+        out = y * torch.sigmoid(y)
+        acc, fixed, dc = 1.1 * acc, 1.1 * fixed, 1.1 * dc
+        fixed = fixed + out.abs() * (5 + 1.2 * y.abs()) * 2.0 ** -23
+    acc, fixed, dc = (t.expand_as(out) for t in (acc, fixed, dc))
+    u = ulp16(out) + fixed
+    err = (got.double() - out).abs()
+    strict = u + c * acc
+    extra = dict(c_needed=((err - u).clamp(min=0) / acc.clamp(min=1e-300)).max().item(), c=c, n_stat=n)
+    if c_dc is None:
+        return check_bound(got, out, strict, report, key, extra=extra)
+    extra.update(strict_worst_err_over_bound=(err / strict).max().item(), c_dc=c_dc,
+                 c_dc_needed=((err - strict).clamp(min=0) / dc.clamp(min=1e-300)).max().item())
+    return check_bound(got, out, strict + c_dc * dc, report, key, extra=extra)
+
+
+def gn_check(got, x, gamma, beta, eps, groups, frames_per_stat, silu, report=None, key="", **kw) -> dict:
+    """GroupNorm of x [NB, HW, C] fp16 with statistics over (C / groups channels, HW, frames_per_stat consecutive images)."""
+    NB, HW, Cc = x.shape
+    shape = (NB // frames_per_stat, frames_per_stat, HW, groups, Cc // groups)
+    gb = [t.double().view(groups, Cc // groups) for t in (gamma, beta)]
+    return norm_check(got.view(shape), x.double().view(shape), (1, 2, 4), *gb, eps, silu, report, key, **kw)
+
+
+def ln_check(got, x, gamma, beta, eps, report=None, key="", **kw) -> dict:
+    """LayerNorm of x [M, C] fp16 over C."""
+    return norm_check(got, x.double(), (1,), gamma.double(), beta.double(), eps, False, report, key, **kw)
+
+
+# ------------------------------------------------------------------------------------------------------------ element-wise steps
+# c of the step bound.  Measured as C_NORM: the largest c any case of test_gpu_elem_edges.py needed was 2.8 (DDIM and CFG + DDIM near
+# alpha-bar = 1); out_temporal needed 2.3, the sinusoid 1.3.
+C_STEP = 4.0
+
+
+def check_step(got, ref, terms, report=None, key="", c: float = C_STEP) -> dict:
+    ref, terms = ref.double(), terms.double()
+    acc = U32 * terms
+    err = (got.double() - ref).abs()
+    extra = dict(c_needed=(err / acc.clamp(min=1e-300)).max().item(), c=c)
+    return check_bound(got, ref, c * acc, report, key, extra=extra)
+
+
+def sqrt32(a: float) -> float:
+    """sqrtf of the float argument, as the host code computes the step coefficients (torch's own fp32 sqrt in the reference)."""
+    return torch.tensor(f32(a), dtype=torch.float32).sqrt().item()
+
+
+def ddim_coef(a: float):
+    """(sqrtf(a), sqrtf(1 - a)) in fp32 from the float alpha-bar."""
+    one_m = (torch.tensor(1.0, dtype=torch.float32) - torch.tensor(f32(a), dtype=torch.float32)).item()
+    return sqrt32(a), sqrt32(one_m)
+
+
+def ddim_invert_ref(x, e, a_prev, a_next):
+    """x_next = sqrt(a_next) x0 + sqrt(1 - a_next) e,  x0 = (x - sqrt(1 - a_prev) e) / sqrt(a_prev)  -> (ref, sum|terms|) fp64."""
+    sp, s1p = ddim_coef(a_prev)
+    sn, s1n = ddim_coef(a_next)
+    x, e = x.double(), e.double()
+    ref = sn * (x - s1p * e) / sp + s1n * e
+    terms = sn * (x.abs() + s1p * e.abs()) / sp + s1n * e.abs()
+    return ref, terms
+
+
+def cfg_ddim_ref(x, eps2, guidance, a_t, a_prev, x_inv=None, blends=None):
+    """x [K, ...], eps2 [2K, ...] = [uncond ; cond]; blends: per item None or (mask_a, mask_b | None) [F, H, W] broadcast over channels,
+    blending towards x_inv.  -> (ref, sum|terms|) fp64."""
+    K = x.shape[0]
+    g = f32(guidance)
+    st, s1t = ddim_coef(a_t)
+    sp, s1p = ddim_coef(a_prev)
+    x, eu, ec = x.double(), eps2[:K].double(), eps2[K:].double()
+    e = eu + g * (ec - eu)
+    te = eu.abs() + abs(g) * (ec.abs() + eu.abs())
+    ref = sp * (x - s1t * e) / st + s1p * e
+    terms = sp * (x.abs() + s1t * te) / st + s1p * te
+    for k, bl in enumerate(blends or [None] * K):
+        if bl is None:
+            continue
+        m = bl[0].double() if bl[1] is None else torch.maximum(bl[0], bl[1]).double()
+        xi = x_inv.double().reshape(ref.shape[1:])
+        ref[k] = xi + m * (ref[k] - xi)
+        terms[k] = xi.abs() + m.abs() * (terms[k] + xi.abs())
+    return ref, terms
+
+
+def _tconv_frames(y, w):
+    """y [B, F, P, Ci], w [Co, Ci, 3] -> [B, F, P, Co]: sum_t w[:, :, t] y[f + t - 1] (zero frames outside)."""
+    yp = F.pad(y, (0, 0, 0, 0, 1, 1))
+    Fr = y.shape[1]
+    return sum(torch.einsum("bfpc,oc->bfpo", yp[:, t:t + Fr], w[:, :, t]) for t in range(3))
+
+
+def out_temporal_ref(y, B, Co, Fr, HW, down=None, up=None, w_full=None, b_full=None):
+    """y [B F HW, ldy] fp16 (Co valid columns) -> (ref, sum|terms|, fixed) [B, Co, F, HW] fp64.  The LoRA path rounds its rank-R
+    intermediate to fp16 as the reference's autocast path does; `fixed` allows that rounding to land one fp16 ulp either way."""
+    y64 = y[:, :Co].double().reshape(B, Fr, HW, Co)
+    fixed = torch.zeros_like(y64)
+    if w_full is not None:
+        w = w_full.double()
+        ref = _tconv_frames(y64, w)
+        terms = _tconv_frames(y64.abs(), w.abs())
+        if b_full is not None:
+            ref, terms = ref + b_full.double(), terms + b_full.double().abs()
+    elif down is not None:
+        mid_exact = _tconv_frames(y64, down.double())
+        mid = mid_exact.half().double()
+        mid_terms = _tconv_frames(y64.abs(), down.double().abs())
+        ua = up.double().abs()
+        ref = y64 + _tconv_frames(mid, up.double())
+        terms = y64.abs() + _tconv_frames(mid.abs(), ua) + _tconv_frames(mid_terms, ua)
+        fixed = _tconv_frames(ulp16(mid_exact), ua)
+    else:
+        ref, terms = y64, y64.abs()
+    perm = (0, 3, 1, 2)
+    return ref.permute(perm), terms.permute(perm), fixed.permute(perm)
+
+
+def rowvec_ref(x, w16, bias, silu_in):
+    """y = W act(x) + b (act = SiLU or identity) -> (ref, sum|terms|, fixed): `fixed` carries the __expf / division error of the SiLU."""
+    x64, w = x.double(), w16.double()
+    a = x64 * torch.sigmoid(x64) if silu_in else x64
+    ref, terms = w @ a, w.abs() @ a.abs()
+    fixed = w.abs() @ (a.abs() * (5 + 1.2 * x64.abs()) * 2.0 ** -23) if silu_in else torch.zeros_like(ref)
+    if bias is not None:
+        ref, terms = ref + bias.double(), terms + bias.double().abs()
+    return ref, terms, fixed
+
+
+def sinusoid_ref(t, c0, flip, freq_shift):
+    """diffusers get_timestep_embedding in fp64 -> (ref, terms): terms = |a| (1 + |z|) + 1 for the argument a = t e^z, whose fp32
+    evaluation (here and in the reference) carries a relative error of a few 2^-24 per unit of |z|, plus sinf / cosf themselves."""
+    half = c0 // 2
+    z = -math.log(10000.0) * torch.arange(half, dtype=torch.float64) / (half - f32(freq_shift))
+    a = f32(t) * torch.exp(z)
+    s, co = torch.sin(a), torch.cos(a)
+    ref = torch.cat([co, s]) if flip else torch.cat([s, co])
+    ta = a.abs() * (1 + z.abs()) + 1
+    return ref, torch.cat([ta, ta])
+
+
+def quick_gelu_ref(x):
+    """x sigmoid(1.702 x) in fp64 from the fp16 input -> (ref, bound): 1 fp16 ulp plus (5 + 2 |x|) 2^-23 |ref| for __expf of the
+    fp32 product 1.702 x and the division."""
+    x64 = x.double()
+    ref = x64 * torch.sigmoid(f32(1.702) * x64)
+    return ref, ulp16(ref) + ref.abs() * (5 + 2 * x64.abs()) * 2.0 ** -23
+
+
+# --------------------------------------------------------------------------------------------------------- blend mask and heat maps
+MASK_TIE = 1e-5  # blend-mask pixels whose fp64 ratio lies this close to th are reported, not asserted
+HEAT_TIE = 1e-4  # heat-map pixels whose fp64 255 a / max lies this close to an integer are reported, not asserted
+
+
+def blend_mask_ratio(maps, word_w, h, w, ntok=77):
+    """spatial_blend.py get_mask in fp64: maps [F, heads, r*r, >= ntok] (one per layer) -> (sum_n map w_n).mean(layers, heads), 3x3 max-pool
+    (stride 1, pad 1), nearest resize to (h, w) with F.interpolate's fp32 source index, divided by the per-frame max.  Returns the ratio [F, h, w] (NaN where the max is 0)."""
+    Fr, heads, rr, _ = maps[0].shape
+    r = int(round(rr ** 0.5))
+    ww = word_w.double()[:ntok].to(maps[0].device)
+    st = torch.stack([(m[..., :ntok].double() * ww).sum(-1) for m in maps]).mean((0, 2)).reshape(Fr, 1, r, r)
+    pooled = F.max_pool2d(st, 3, 1, 1)[:, 0]
+    mk = pooled[:, nearest_index(r, h).to(pooled.device)][:, :, nearest_index(r, w).to(pooled.device)]
+    return mk / mk.amax((-2, -1), keepdim=True)
+
+
+def nearest_index(n_in: int, n_out: int) -> torch.Tensor:
+    """F.interpolate(mode="nearest") source index as torch computes it for fp16 / fp32 tensors: min(floor(dst * ((float)n_in / n_out)),
+    n_in - 1) in fp32.  (On fp64 tensors torch uses a double scale, which differs at some sizes: the reference's maps are fp16 / fp32.)"""
+    scale = torch.tensor(n_in, dtype=torch.float32) / n_out
+    return torch.floor(torch.arange(n_out, dtype=torch.float32) * scale).long().clamp(max=n_in - 1)
+
+
+def check_mask(got, ratio, th, report=None, key="") -> dict:
+    """Every pixel equal to ratio > th (NaN -> 0), except those with |ratio - th| <= MASK_TIE (counted as n_near, not asserted)."""
+    want = ratio.gt(th).to(got.dtype)
+    near = (ratio - th).abs() <= MASK_TIE
+    bad = (got != want) & ~near
+    stats = dict(n=got.numel(), n_near=int(near.sum().item()), ones=want.mean().item(), mismatches=int(bad.sum().item()))
+    _record(report, key, stats)
+    assert stats["mismatches"] == 0, f"{key}: {stats['mismatches']} mask pixels differ from the fp64 reference ({stats})"
+    return stats
+
+
+def heatmap_values(maps, ntok):
+    """fz_cross_heatmaps in fp64: maps [F, heads, rr, ldm] -> 255 a / max over pixels, a = sum over maps and heads; [F, ntok, rr].
+    A column whose maximum is 0 gives 0."""
+    a = torch.stack([m[..., :ntok].double() for m in maps]).sum((0, 2)).transpose(1, 2)  # [F, ntok, rr]
+    mx = a.amax(-1, keepdim=True)
+    return torch.where(mx > 0, 255 * a / mx.clamp(min=1e-300), torch.zeros_like(a))
+
+
+def check_heatmaps(got, v, report=None, key="") -> dict:
+    """got uint8 [F, ntok, rr] == floor(min(255, v)) except where v is within HEAT_TIE of an integer (there: within 1)."""
+    want = v.clamp(max=255).floor()
+    near = (v - v.round()).abs() <= HEAT_TIE
+    g = got.double()
+    bad = ((g != want) & ~near) | ((g - v).abs() > 1)
+    stats = dict(n=got.numel(), n_near=int(near.sum().item()), mismatches=int(bad.sum().item()))
+    _record(report, key, stats)
+    assert stats["mismatches"] == 0, f"{key}: {stats['mismatches']} heat-map pixels differ from the fp64 reference ({stats})"
+    return stats

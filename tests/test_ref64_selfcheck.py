@@ -1,10 +1,15 @@
 """CPU proof that the fp64 comparators of tests/_ref64.py are tight enough: they accept a correctly rounded fp16 result and reject the same
 result with one element moved by 3 ulps, a bias applied one column off, or one 64-wide k-block missing (and, for attention, probabilities
-normalised slightly differently or one 64-key block missing).  No GPU: everything here is fp64 on the CPU."""
+normalised slightly differently or one 64-key block missing).  The norm bounds reject a variance over n - 1, eps outside the square root,
+per-frame instead of joint-frame statistics and the fused-shift rounding on a constant row; the softmax bound a scale one fp16 ulp off;
+the mask and heat-map checks a resize index off by one (and the integer nearest index) and a white all-zero column; the step bound CFG
+guidance applied to the wrong half.  No GPU: everything here is fp64 on the CPU."""
 import pytest
 import torch
+import torch.nn.functional as F
 
-from _ref64 import check_attn, check_probs, check_tap, gemm_ref, softmax64, ulp16
+from _ref64 import (blend_mask_ratio, cfg_ddim_ref, check_attn, check_heatmaps, check_mask, check_probs, check_step, check_tap, ddim_invert_ref,
+                    gemm_ref, gn_check, heatmap_values, ln_check, nearest_index, softmax64, ulp16)
 
 
 def rnd(*shape, seed=0, scale=1.0):
@@ -98,3 +103,152 @@ def test_probs_reject_other_normalisation():
     q[:, -1] = 0
     with pytest.raises(AssertionError, match="out of bound"):
         check_probs(q.half(), p)
+
+
+# ------------------------------------------------------------------------------------------------------- normalisation, steps, masks
+def ln_case(M=12, C=64, sigma=1.0, mean=0.5, seed=20):
+    x = (rnd(M, C, seed=seed) * sigma + mean).half()
+    g, b = 1 + 0.3 * rnd(C, seed=seed + 1), 0.2 * rnd(C, seed=seed + 2)
+    return x, g, b
+
+
+def ln64(x, g, b, eps=1e-5, unbiased=False, eps_outside=False):
+    x64 = x.double()
+    mu = x64.mean(-1, keepdim=True)
+    var = x64.var(-1, unbiased=unbiased, keepdim=True)
+    den = var.sqrt() + eps if eps_outside else (var + eps).sqrt()
+    return (x64 - mu) / den * g.double() + b.double()
+
+
+def test_norm_accepts_correct_rounding():
+    x, g, b = ln_case()
+    ln_check(ln64(x, g, b).half(), x, g, b, 1e-5)
+    xg = (rnd(8, 16, 64, seed=30) + rnd(8, 1, 64, seed=31)).half()
+    gg, bg = 1 + 0.3 * rnd(64, seed=32), 0.2 * rnd(64, seed=33)
+    for fps, silu in [(1, False), (4, True), (8, False)]:
+        y = F.group_norm(xg.double().view(8 // fps, fps, 16, 64).permute(0, 3, 1, 2), 8, gg.double(), bg.double(), 1e-5)
+        y = y.permute(0, 2, 3, 1).reshape(8, 16, 64)
+        gn_check((F.silu(y) if silu else y).half(), xg, gg, bg, 1e-5, 8, fps, silu)
+
+
+def test_norm_rejects_unbiased_variance():
+    x, g, b = ln_case()
+    with pytest.raises(AssertionError, match="out of bound"):
+        ln_check(ln64(x, g, b, unbiased=True).half(), x, g, b, 1e-5)
+
+
+def test_norm_rejects_eps_outside_sqrt():
+    x, g, b = ln_case(sigma=0.02)  # sigma^2 = 4e-4: eps = 1e-5 outside the root moves rstd by about 1 %
+    with pytest.raises(AssertionError, match="out of bound"):
+        ln_check(ln64(x, g, b, eps_outside=True).half(), x, g, b, 1e-5)
+
+
+def test_norm_rejects_per_frame_statistics():
+    xg = (rnd(8, 16, 64, seed=30) + 0.5 * rnd(8, 1, 64, seed=31)).half()
+    gg, bg = 1 + 0.3 * rnd(64, seed=32), 0.2 * rnd(64, seed=33)
+    y = F.group_norm(xg.double().permute(0, 2, 1), 8, gg.double(), bg.double(), 1e-5).permute(0, 2, 1)  # frames_per_stat = 1
+    gn_check(y.half(), xg, gg, bg, 1e-5, 8, 1, False)
+    with pytest.raises(AssertionError, match="out of bound"):
+        gn_check(y.half(), xg, gg, bg, 1e-5, 8, 4, False)
+
+
+def fma32(a, b, c):
+    """fmaf on fp32 tensors: the product is exact in fp64, one rounding of the sum (to fp64, then fp32: a double rounding that cannot
+    matter at the size of the errors checked here)."""
+    return (a.double() * b.double() + c.double()).float()
+
+
+@pytest.mark.parametrize("C", [64, 320, 768, 1280])
+def test_norm_rejects_fused_shift_on_constant_row(C):
+    """The LayerNorm of a constant row is beta exactly.  y = fma(fma(v, rstd, shift), gamma, beta) with shift = fp32(-mean * rstd) carries
+    the rounding of shift (2^-24 |mean| rstd, rstd = eps^-1/2 = 316 here) into beta."""
+    vals = torch.tensor([-150.0, -37.5, 100.0, 199.0, 0.3, 3.0])
+    x = vals[:, None].expand(len(vals), C).half()
+    g, b = 1 + 0.3 * rnd(C, seed=40), 0.02 * rnd(C, seed=41)
+    ln_check(b.expand(len(vals), C).half(), x, g, b, 1e-5)  # the exact answer passes
+    v = x.float()
+    inv_c = torch.tensor(1.0 / C, dtype=torch.float32)
+    s = v.sum(-1, keepdim=True)
+    rstd = (torch.zeros(len(vals), 1) + torch.tensor(1e-5, dtype=torch.float32)).rsqrt()
+    shift = (-s * inv_c) * rstd
+    y = fma32(fma32(v, rstd.expand_as(v), shift.expand_as(v)), g.expand_as(v), b.expand_as(v))
+    with pytest.raises(AssertionError, match="out of bound"):
+        ln_check(y.half(), x, g, b, 1e-5)
+
+
+def test_probs_reject_scale_one_fp16_ulp_off():
+    x = (rnd(16, 512, seed=50) * 40).half()
+    s = 512 ** -0.5
+    p = softmax64(x.double() * s)
+    check_probs(p.half(), p)
+    with pytest.raises(AssertionError, match="out of bound"):
+        check_probs(softmax64(x.double() * s * (1 + 2.0 ** -10)).half(), p)
+
+
+def mask_maps(Fr=2, heads=4, r=16, seed=60):
+    return [torch.softmax(rnd(Fr, heads, r * r, 80, seed=seed + i) * 2, -1).half() for i in range(3)]
+
+
+def test_mask_rejects_index_off_by_one():
+    maps = mask_maps()
+    ww = torch.zeros(77)
+    ww[[2, 76]] = 1
+    h, w = 64, 40
+    ratio = blend_mask_ratio(maps, ww, h, w)
+    check_mask(ratio.gt(0.5).float(), ratio, 0.5)
+    # the same pipeline with the nearest-resize source row one further down
+    st = torch.stack([(m[..., :77].double() * ww.double()).sum(-1) for m in maps]).mean((0, 2)).reshape(2, 1, 16, 16)
+    pooled = F.max_pool2d(st, 3, 1, 1)[:, 0]
+    sy = (nearest_index(16, h) + 1).clamp(max=15)
+    sx = nearest_index(16, w)
+    mk = pooled[:, sy][:, :, sx]
+    shifted = mk / mk.amax((-2, -1), keepdim=True)
+    with pytest.raises(AssertionError, match="differ"):
+        check_mask(shifted.gt(0.5).float(), ratio, 0.5)
+
+
+def test_mask_rejects_integer_resize_index():
+    """(y * r) / h in integers differs from F.interpolate's floor(y * (float)(r / h)) at r = 16, h = 82; a map that ramps along y with th
+    between the two source rows makes that row of the mask differ."""
+    r, h = 16, 82
+    ramp = torch.arange(r, dtype=torch.float64).repeat_interleave(r) / r  # row y of the r x r grid holds y / r
+    maps = [torch.zeros(1, 1, r * r, 80, dtype=torch.float16)]
+    maps[0][0, 0, :, 5] = ramp.half()
+    ww = torch.zeros(77)
+    ww[5] = 1
+    ratio = blend_mask_ratio(maps, ww, h, h)
+    pooled = F.max_pool2d(ramp.view(1, 1, r, r), 3, 1, 1)[0, 0, :, 0]
+    ours = (torch.arange(h) * r // h).clamp(max=r - 1)
+    torch_idx = nearest_index(r, h)
+    assert torch.equal(torch_idx, F.interpolate(torch.arange(r, dtype=torch.float32).view(1, 1, r), size=h).view(-1).long())
+    y = int((ours != torch_idx).nonzero()[0])
+    th = 0.5 * (pooled[ours[y]] + pooled[torch_idx[y]]).item() / pooled.max().item()
+    mk = pooled[ours][:, None].expand(h, h)[None]
+    with pytest.raises(AssertionError, match="differ"):
+        check_mask((mk / mk.max()).gt(th).float(), ratio, th)
+
+
+def test_heatmaps_reject_white_zero_column():
+    maps = [torch.softmax(rnd(2, 4, 64, 80, seed=70), -1).half()]
+    maps[0][..., 9] = 0
+    v = heatmap_values(maps, 77)
+    good = v.clamp(max=255).floor().to(torch.uint8)
+    check_heatmaps(good, v)
+    bad = good.clone()
+    bad[:, 9] = 255  # fminf(255, 0/0) on a column whose maximum is 0
+    with pytest.raises(AssertionError, match="differ"):
+        check_heatmaps(bad, v)
+
+
+def test_step_rejects_guidance_on_wrong_half():
+    K = 3
+    x, eps2, x_inv = rnd(K, 4, 2, 5, 6, seed=80), rnd(2 * K, 4, 2, 5, 6, seed=81), rnd(1, 4, 2, 5, 6, seed=82)
+    blends = [((rnd(2, 5, 6, seed=83) > 0).float(), None), None, ((rnd(2, 5, 6, seed=84) > 0).float(), (rnd(2, 5, 6, seed=85) > 0).float())]
+    ref, terms = cfg_ddim_ref(x, eps2, 7.5, 0.3, 0.4, x_inv, blends)
+    check_step(ref.float(), ref, terms)
+    swapped = torch.cat([eps2[K:], eps2[:K]])
+    wrong, _ = cfg_ddim_ref(x, swapped, 7.5, 0.3, 0.4, x_inv, blends)
+    with pytest.raises(AssertionError, match="out of bound"):
+        check_step(wrong.float(), ref, terms)
+    inv, inv_terms = ddim_invert_ref(x, eps2[:K], 0.3, 0.4)
+    check_step(inv.float(), inv, inv_terms)
