@@ -294,19 +294,40 @@ static int launch_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
   return FZ_OK;
 }
 
-static int pick_block_n(int gemm_cols, int mode, int forced, int m_tiles) {
+// Skip tensors that fold_residuals() turns into extra k-blocks (all present ones, or none): row-major epilogue without V^T, and every
+// skip tensor TMA-addressable (16-byte base and row stride).
+static int n_foldable(const TapGemmParams& p) {
+  if (p.mode != FZ_EPI_ROWMAJOR || p.vt_col_start != INT_MAX) return 0;
+  const __half* rs[2] = {p.residual, p.residual2};
+  const long long lds[2] = {p.ldr, p.ldr2};
+  int n = 0;
+  for (int i = 0; i < 2; ++i) {
+    if (!rs[i]) continue;
+    if ((reinterpret_cast<uintptr_t>(rs[i]) & 15) != 0 || lds[i] % 8 != 0) return 0;
+    ++n;
+  }
+  return n;
+}
+
+// k_main = taps x k-blocks of the contraction; p holds the epilogue (fill_epilogue) so the folded skip k-blocks can be counted.
+static int pick_block_n(const TapGemmParams& p, int gemm_cols, int forced, int m_tiles, int k_main) {
   if (forced > 0) return forced;
   static const int cands[] = {256, 160, 128, 64, 32, 16};
-  if (mode == FZ_EPI_GEGLU) return (gemm_cols % 256 == 0) ? 256 : ((gemm_cols % 160 == 0) ? 160 : ((gemm_cols % 128 == 0) ? 128 : ((gemm_cols % 64 == 0) ? 64 : 32)));
-  // cost model: a tile costs ~ BLOCK_N MMA columns (+ a fixed part), tiles run in waves of one per SM.
+  if (p.mode == FZ_EPI_GEGLU) return (gemm_cols % 256 == 0) ? 256 : ((gemm_cols % 160 == 0) ? 160 : ((gemm_cols % 128 == 0) ? 128 : ((gemm_cols % 64 == 0) ? 64 : 32)));
+  // Cost model: tiles run in waves of one per SM.  Time of a 128 x bn tile with k k-blocks (folded skip blocks included), fitted to
+  // per-shape timings of the UNet's linears, 3x3 convs and temporal convs on an H100 80 GB HBM3 (700 W):  bn k + 24 bn + 110 k + 0.15 bn^2.
+  // Beyond the MMA term (bn k), the per-tile parts that grow with bn (epilogue, and the ring holding fewer stages of a wider W tile)
+  // make narrow tiles win at short K: BLOCK_N 64 for the K <= 640 linears, 160 for the 9-tap convs.
   const int sms = num_sms();
+  const int n_fold = n_foldable(p);
   int best = 16;
   double best_cost = 1e30;
   for (int bn : cands) {
     const long long n_tiles = (gemm_cols + bn - 1) / bn;
     const long long tiles = n_tiles * m_tiles;
     const long long waves = (tiles + sms - 1) / sms;
-    const double cost = static_cast<double>(waves) * (bn + 24.0);
+    const double k = k_main + n_fold * ((bn + kBlockK - 1) / kBlockK);
+    const double cost = static_cast<double>(waves) * (bn * k + 24.0 * bn + 110.0 * k + 0.15 * bn * bn);
     if (cost < best_cost - 1e-9) { best_cost = cost; best = bn; }
   }
   return best;
@@ -344,11 +365,9 @@ static int eye_table(__half** out, cudaStream_t stream) {
 static int fold_residuals(TapGemmParams& p, int bn, cudaStream_t stream) {
   p.n_res = 0;
   p.res_kblocks = 0;
-  if (p.mode != FZ_EPI_ROWMAJOR || p.vt_col_start != INT_MAX || (!p.residual && !p.residual2)) return FZ_OK;
+  if (n_foldable(p) == 0) return FZ_OK;  // none, or not TMA-addressable: epilogue path
   const __half* rs[2] = {p.residual, p.residual2};
   const long long lds[2] = {p.ldr, p.ldr2};
-  for (int i = 0; i < 2; ++i)
-    if (rs[i] && ((reinterpret_cast<uintptr_t>(rs[i]) & 15) != 0 || lds[i] % 8 != 0)) return FZ_OK;  // not TMA-addressable: epilogue path
   __half* eye = nullptr;
   if (int rc = eye_table(&eye, stream)) return rc;
   {
@@ -371,9 +390,9 @@ static int fold_residuals(TapGemmParams& p, int bn, cudaStream_t stream) {
   return FZ_OK;
 }
 
-static int dispatch_tapgemm(TapGemmParams& p, int gemm_cols, int forced_bn, cudaStream_t stream) {
+// bn: the caller's pick_block_n() result (its W tensor map already has a {64, bn} box)
+static int dispatch_tapgemm(TapGemmParams& p, int gemm_cols, int bn, cudaStream_t stream) {
   if (int rc = check_single_device()) return rc;
-  const int bn = pick_block_n(gemm_cols, p.mode, forced_bn, p.m_tiles);
   p.n_tiles = (gemm_cols + bn - 1) / bn;
   if (int rc = fold_residuals(p, bn, stream)) return rc;
   switch (bn) {
@@ -439,7 +458,7 @@ extern "C" int fz_gemm_f16(const void* A, long long lda, const void* W, long lon
   const int rc0 = fill_epilogue(p, epi, M, N);
   if (rc0) return rc0;
   p.m_tiles = (M + kBlockM - 1) / kBlockM;
-  const int bn = pick_block_n(N, p.mode, force_block_n, p.m_tiles);
+  const int bn = pick_block_n(p, N, force_block_n, p.m_tiles, (K + kBlockK - 1) / kBlockK);
   {
     uint64_t dims[3] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N), 1};
     uint64_t strides[2] = {static_cast<uint64_t>(ldw), static_cast<uint64_t>(ldw) * N};
@@ -508,7 +527,7 @@ static int conv3x3_impl(const void* x, long long ldx, int NB, int H, int W, int 
   }
   p.rows_per_tile = bw * bh * bn_img;
   p.m_tiles = M / p.rows_per_tile;
-  const int bn = pick_block_n(Cout, p.mode, force_block_n, p.m_tiles);
+  const int bn = pick_block_n(p, Cout, force_block_n, p.m_tiles, 9 * ((Cin + kBlockK - 1) / kBlockK));
   {
     uint64_t dims[3] = {(uint64_t)Cin, (uint64_t)Cout, 9};
     uint64_t strides[2] = {(uint64_t)Cin, (uint64_t)Cin * Cout};
@@ -561,7 +580,7 @@ static int tconv3_impl(const void* x, long long ldx, int B, int F, int HW, int C
   for (int t = 0; t < 3; ++t) { p.tap_off[t][2] = t - 1 + halo; }
   p.rows_per_tile = bp * bf;
   p.m_tiles = M / p.rows_per_tile;
-  const int bn = pick_block_n(Cout, p.mode, force_block_n, p.m_tiles);
+  const int bn = pick_block_n(p, Cout, force_block_n, p.m_tiles, 3 * ((Cin + kBlockK - 1) / kBlockK));
   {
     uint64_t dims[3] = {(uint64_t)Cin, (uint64_t)Cout, 3};
     uint64_t strides[2] = {(uint64_t)Cin, (uint64_t)Cin * Cout};
