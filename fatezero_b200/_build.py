@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfatezero_b200.so")
-SOURCES = ["fz_capi.cu", "fz_gemm.cu", "fz_elem.cu", "fz_attn.cu", "fz_p2p.cu"]
+SOURCES = ["fz_capi.cu", "fz_gemm.cu", "fz_elem.cu", "fz_attn.cu", "fz_p2p.cu", "fz_clip.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "--use_fast_math" if False else "-DFZ_NO_FAST_MATH"]

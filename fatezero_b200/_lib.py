@@ -106,6 +106,13 @@ SIGNATURES = {
     "fz_embed_tokens_f16": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     "fz_quick_gelu_f16": [c_void_p, c_ll, c_void_p],
     "fz_cross_heatmaps": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "fz_frames_to_u8": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p],
+    "fz_resize_bicubic_u8": [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                             c_void_p, c_void_p, c_void_p],
+    "fz_clip_patchify_f16": [c_void_p, c_int, c_int, c_int, c_int, c_int, C.POINTER(c_float), C.POINTER(c_float), c_void_p, c_void_p],
+    "fz_clip_embed_f16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_int, c_void_p, c_void_p],
+    "fz_clip_scores": [c_void_p, c_void_p, c_int, c_int, c_int, C.POINTER(c_int), C.POINTER(c_int), c_int, c_float, c_void_p, c_void_p,
+                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "fz_device_check": [],
     "fz_init": [c_void_p],
     "fz_version": [],
@@ -115,7 +122,8 @@ _lib = None
 launch_count = 0     # C-ABI compute calls issued
 kernel_launches = 0  # kernels of this library launched (bench.py reports the delta over its timed region)
 KERNELS_PER_CALL = {"fz_groupnorm_nhwc_f16": 2, "fz_groupnorm_batched_nhwc_f16": 2, "fz_p2p_alloc": 0, "fz_p2p_free": 0, "fz_p2p_export": 0, "fz_p2p_import": 0,
-                    "fz_p2p_unimport": 0, "fz_init": 0}  # stats + apply (plus one memset); every other entry point launches one kernel
+                    "fz_p2p_unimport": 0, "fz_init": 0, "fz_resize_bicubic_u8": 2}  # stats + apply (plus one memset); horizontal + vertical
+# pass; every other entry point launches one kernel
 
 
 def load():

@@ -62,20 +62,28 @@ class ClipTextEngine:
         B, L = input_ids.shape
         if L > self.L:
             raise ValueError(f"{L} tokens > max_position_embeddings {self.L}")
-        C, heads, d = self.C, self.heads, self.d
-        ld = (L + 7) // 8 * 8
         with torch.cuda.device(self.dev):
             x = ops.embed_tokens(self.tok, self.pos, input_ids.to(self.dev))
-            vt = torch.zeros((B, heads, d, ld), dtype=f16, device=self.dev)
-            for ly in self.layers:
-                hn = ops.layernorm(x, *ly["ln1"], eps=self.eps)
-                qk = ops.gemm(hn, ly["qkv_w"], bias=ly["qkv_b"], vt=dict(out=vt, col_start=2 * C, S=L, d=d, heads=heads, ld=ld))
-                o = torch.empty((B * L, C), dtype=f16, device=self.dev)
-                ops.attention(qk[:, :C], qk[:, C:], vt, o, S_q=L, keys_per_slot=L, n_src=B, d=d, heads=heads, F=1, BF=B, scale=d ** -0.5,
-                              src_index=[list(range(B))], causal=True)
-                x = ops.gemm(o, ly["out_w"], bias=ly["out_b"], residual=x)
-                hn = ops.layernorm(x, *ly["ln2"], eps=self.eps)
-                m = ops.quick_gelu_(ops.gemm(hn, ly["fc1_w"], bias=ly["fc1_b"]))
-                x = ops.gemm(m, ly["fc2_w"], bias=ly["fc2_b"], residual=x)
+            x = transformer_blocks(x, self.layers, B, L, self.C, self.heads, self.eps, causal=True)
             out = ops.layernorm(x, *self.ln_f, eps=self.eps)
-        return (out.float().view(B, L, C),)
+        return (out.float().view(B, L, self.C),)
+
+
+def transformer_blocks(x: torch.Tensor, layers, B: int, L: int, C: int, heads: int, eps: float, causal: bool) -> torch.Tensor:
+    """The pre-LN CLIP residual blocks on the current device: x [B*L, C] fp16 (B <= 64 sequences of L tokens, fz_attention_f16's row
+    limit) through {LN, self-attention, LN, quick_gelu MLP} per layer dict (ln1, ln2, qkv_w / qkv_b with q | k | v rows, out_w / out_b,
+    fc1_w / fc1_b, fc2_w / fc2_b)."""
+    d = C // heads
+    ld = (L + 7) // 8 * 8
+    vt = torch.zeros((B, heads, d, ld), dtype=f16, device=x.device)
+    for ly in layers:
+        hn = ops.layernorm(x, *ly["ln1"], eps=eps)
+        qk = ops.gemm(hn, ly["qkv_w"], bias=ly["qkv_b"], vt=dict(out=vt, col_start=2 * C, S=L, d=d, heads=heads, ld=ld))
+        o = torch.empty((B * L, C), dtype=f16, device=x.device)
+        ops.attention(qk[:, :C], qk[:, C:], vt, o, S_q=L, keys_per_slot=L, n_src=B, d=d, heads=heads, F=1, BF=B, scale=d ** -0.5,
+                      src_index=[list(range(B))], causal=causal)
+        x = ops.gemm(o, ly["out_w"], bias=ly["out_b"], residual=x)
+        hn = ops.layernorm(x, *ly["ln2"], eps=eps)
+        m = ops.quick_gelu_(ops.gemm(hn, ly["fc1_w"], bias=ly["fc1_b"]))
+        x = ops.gemm(m, ly["fc2_w"], bias=ly["fc2_b"], residual=x)
+    return x

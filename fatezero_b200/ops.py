@@ -309,6 +309,84 @@ def quick_gelu_(x: torch.Tensor) -> torch.Tensor:
     return x
 
 
+def frames_to_u8(x: torch.Tensor) -> torch.Tensor:
+    """decoded frames [N, 3, H, W] fp32 / fp16 in [-1, 1] -> uint8 [N, H, W, 3], bitwise numpy_to_pil's bytes."""
+    if x.dtype not in (torch.float32, f16):
+        raise TypeError(f"fatezero_b200.ops.frames_to_u8: expected float32 or float16, got {x.dtype}")
+    _chk(x, x.dtype, "frames_to_u8")
+    N, c, H, W = x.shape
+    if c != 3:
+        raise ValueError(f"fatezero_b200.ops.frames_to_u8: {c} channels (RGB expected)")
+    x = x.contiguous()
+    out = torch.empty((N, H, W, 3), dtype=torch.uint8, device=x.device)
+    _lib.call("fz_frames_to_u8", _p(x), int(x.dtype == f16), _p(out), N, H, W, _stream())
+    return out
+
+
+def resize_bicubic_u8(img: torch.Tensor, tables, crop_bottom_square: bool = False) -> torch.Tensor:
+    """img [N, H, W, 3] uint8 -> [N, Ho, Wo, 3] uint8 with PIL's bicubic resample.  tables: device dict(kx, bx, ky, by) of
+    clip_eval.resize_tables for the (cropped) input size."""
+    _chk(img, torch.uint8, "resize_bicubic_u8")
+    N, H, W, c = img.shape
+    assert c == 3 and img.is_contiguous()
+    kx, bx, ky, by = tables["kx"], tables["bx"], tables["ky"], tables["by"]
+    for t in (kx, bx, ky, by):
+        _chk(t, torch.int32, "resize_bicubic_u8")
+        assert t.is_contiguous()
+    Wo, Ho = kx.shape[0], ky.shape[0]
+    hc = W if crop_bottom_square and H > W else H
+    tmp = torch.empty((N, hc, Wo, 3), dtype=torch.uint8, device=img.device)
+    out = torch.empty((N, Ho, Wo, 3), dtype=torch.uint8, device=img.device)
+    _lib.call("fz_resize_bicubic_u8", _p(img), N, H, W, int(crop_bottom_square), _p(kx), _p(bx), kx.shape[1], Wo, _p(ky), _p(by), ky.shape[1],
+              Ho, _p(tmp), _p(out), _stream())
+    return out
+
+
+def clip_patchify(img: torch.Tensor, res: int, patch: int, mean: Sequence[float], std: Sequence[float]) -> torch.Tensor:
+    """resized uint8 [N, Hr, Wr, 3] -> CenterCrop(res) + ToTensor + Normalize as fp16 conv1 im2col rows [N*(res/patch)^2, 3*patch^2]."""
+    _chk(img, torch.uint8, "clip_patchify")
+    N, Hr, Wr, c = img.shape
+    assert c == 3 and img.is_contiguous()
+    g = res // patch if patch > 0 else 0
+    out = torch.empty((max(N * g * g, 1), 3 * patch * patch), dtype=f16, device=img.device)
+    _lib.call("fz_clip_patchify_f16", _p(img), N, Hr, Wr, int(res), int(patch), (C.c_float * 3)(*map(float, mean)),
+              (C.c_float * 3)(*map(float, std)), _p(out), _stream())
+    return out
+
+
+def clip_embed(patches: torch.Tensor, class_emb: torch.Tensor, pos_emb: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float,
+               N: int) -> torch.Tensor:
+    """patch-GEMM rows [N*(T-1), C] fp16 -> ln_pre(cat(class, patches) + pos) [N*T, C] fp16 (T = pos_emb rows)."""
+    _chk(patches, f16, "clip_embed")
+    for t in (class_emb, pos_emb, gamma, beta):
+        _chk(t, torch.float32, "clip_embed")
+    T, Cc = pos_emb.shape
+    assert patches.is_contiguous() and patches.shape == (N * (T - 1), Cc)
+    out = torch.empty((N * T, Cc), dtype=f16, device=patches.device)
+    _lib.call("fz_clip_embed_f16", _p(patches), _p(class_emb.contiguous()), _p(pos_emb.contiguous()), _p(gamma), _p(beta), float(eps), N, T, Cc,
+              _p(out), _stream())
+    return out
+
+
+def clip_scores(img: torch.Tensor, txt: torch.Tensor, clip_frames: Sequence[int], pairs: Sequence[Sequence[int]], scale: float) -> dict:
+    """img [N, D] / txt [P, D] fp32 features; clip_frames [K]; pairs [K] x (source row, target row) -> dict of fp32 device tensors
+    (success int32): img_norm, txt_norm, logits [N, 2], probs [N, 2], success, margin, cosine [N], clip_mean [K]."""
+    _chk(img, torch.float32, "clip_scores"); _chk(txt, torch.float32, "clip_scores")
+    N, D = img.shape
+    P = txt.shape[0]
+    assert txt.shape[1] == D and img.is_contiguous() and txt.is_contiguous()
+    K = len(clip_frames)
+    dev = img.device
+    o = dict(img_norm=torch.empty(N, device=dev), txt_norm=torch.empty(P, device=dev), logits=torch.empty(N, 2, device=dev),
+             probs=torch.empty(N, 2, device=dev), success=torch.empty(N, dtype=torch.int32, device=dev), margin=torch.empty(N, device=dev),
+             cosine=torch.empty(N, device=dev), clip_mean=torch.empty(max(K, 1), device=dev))
+    fr = (C.c_int * max(K, 1))(*[int(f) for f in clip_frames])
+    pr = (C.c_int * max(2 * K, 1))(*[int(v) for pq in pairs for v in pq])
+    _lib.call("fz_clip_scores", _p(img), _p(txt), N, P, D, fr, pr, K, float(scale), *(_p(o[k]) for k in
+              ("img_norm", "txt_norm", "logits", "probs", "success", "margin", "cosine", "clip_mean")), _stream())
+    return o
+
+
 def cross_heatmaps(maps: Sequence[torch.Tensor], ntok: int) -> torch.Tensor:
     """maps: cross-attention running sums [F, heads, r*r, ld] (fp16 or fp32) of ONE resolution -> uint8 [F, ntok, r, r] heat maps."""
     m0 = maps[0]

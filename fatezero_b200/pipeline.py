@@ -227,6 +227,22 @@ class SpatioTemporalStableDiffusionPipeline:
             image = image.transpose(0, 2, 3, 1)
         return image
 
+    @torch.no_grad()
+    def decode_latents_u8(self, latents):
+        """decode_latents + numpy_to_pil without leaving the device: uint8 frames [b, f, H, W, 3] for video latents [b, 4, f, h, w]
+        ([N, H, W, 3] for image latents), bitwise the bytes of the PIL frames.  Needs the sm_90a VAE engine (fatezero_b200.vae)."""
+        eng = self._vae_engine()
+        if eng is None:
+            raise RuntimeError("decode_latents_u8 runs on the sm_90a VAE engine: the pipeline's vae is not a fatezero_b200.vae.AutoencoderKL "
+                               "nor an AutoencoderKL-shaped module on a CUDA device")
+        is_video = latents.dim() == 5
+        b = latents.shape[0]
+        latents = 1 / 0.18215 * latents
+        if is_video:
+            latents = latents.permute(0, 2, 1, 3, 4).reshape(-1, *latents.shape[1:2], *latents.shape[3:])
+        frames = torch.cat([ops.frames_to_u8(eng.decode(chunk)) for chunk in torch.split(latents, 16, dim=0)], dim=0)
+        return frames.reshape(b, -1, *frames.shape[1:]) if is_video else frames
+
     def prepare_extra_step_kwargs(self, generator, eta):
         keys = set(inspect.signature(self.scheduler.step).parameters.keys())
         out = {}

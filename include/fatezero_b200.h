@@ -200,6 +200,41 @@ int fz_cross_heatmaps(const void* const* maps, int num_maps, int maps_f32, int F
                       fz_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * CLIP evaluation of edited clips (paths relative to the reference's CLIP/ directory): frame accuracy and temporal consistency of
+ * frame_acc_tem_con.py:11-54 with a CLIP ViT (clip/model.py:206-238 image tower, :343-372 text tower and logits).  The transformer
+ * blocks run on fz_gemm_f16 / fz_attention_f16 / fz_layernorm_f16 / fz_quick_gelu_f16; these are the pieces around them.
+ * --------------------------------------------------------------------------------------------------------- */
+#define FZ_CLIP_MAX_SIDE 8192 /* largest input or resized side, in pixels                                          */
+#define FZ_CLIP_MAX_CLIPS 256 /* clips per fz_clip_scores launch                                                    */
+/* decode_latents + numpy_to_pil (pipelines/stable_diffusion.py:297-319,566-576) on the device: x [N,3,H,W] fp32 (x_f16 = 0) or fp16 in
+ * [-1,1] -> out [N,H,W,3] uint8 = round_half_even(clamp(x / 2 + 0.5, 0, 1) * 255), the fp16 case evaluated in fp16 as torch does. */
+int fz_frames_to_u8(const void* x, int x_f16, unsigned char* out, int N, int H, int W, fz_stream_t stream);
+/* PIL Image.resize(BICUBIC) as torchvision's Resize calls it (clip/clip.py:79-86; Pillow libImaging/Resample.c, 8 bits per channel):
+ * in [N,H,W,3] uint8 (crop_bottom_square: a frame with H > W is first cropped to its bottom W x W square, frame_acc_tem_con.py:11-16)
+ * -> out [N,Ho,Wo,3].  kx [Wo, kw_x] / ky [Ho, kw_y]: device int32 weights with 22 fractional bits; bx [Wo][2] / by [Ho][2]: device int32
+ * (first input pixel, tap count) per output pixel (host tables: fatezero_b200.clip_eval.resize_coeffs).  tmp: [N, H', Wo, 3] uint8 scratch
+ * for the horizontal pass (H' = the cropped height). */
+int fz_resize_bicubic_u8(const unsigned char* in, int N, int H, int W, int crop_bottom_square, const int* kx, const int* bx, int kw_x, int Wo,
+                         const int* ky, const int* by, int kw_y, int Ho, unsigned char* tmp, unsigned char* out, fz_stream_t stream);
+/* CenterCrop(res) + ToTensor + Normalize(mean3, std3) (clip/clip.py:79-86), rounded to fp16 (model.py:340 `image.type(self.dtype)`), written
+ * as the im2col rows of conv1 (model.py:222): img [N,Hr,Wr,3] uint8 -> out [N*(res/patch)^2, 3*patch*patch] fp16, column c*patch^2 + ky*patch
+ * + kx.  mean3 / std3: HOST arrays. */
+int fz_clip_patchify_f16(const unsigned char* img, int N, int Hr, int Wr, int res, int patch, const float* mean3, const float* std3, void* out,
+                         fz_stream_t stream);
+/* model.py:223-227: out[n*T + t] = ln_pre((t == 0 ? class_emb : patches[n*(T-1) + t-1]) + pos_emb[t]) with fp32 statistics, fp16 out.
+ * patches [N*(T-1), C] fp16 (the conv1 GEMM), class_emb [C], pos_emb [T, C], gamma / beta [C] fp32; C % 8 == 0, C <= 1024. */
+int fz_clip_embed_f16(const void* patches, const float* class_emb, const float* pos_emb, const float* gamma, const float* beta, float eps,
+                      int N, int T, int C, void* out, fz_stream_t stream);
+/* Scoring head, fp32, one launch (frame_acc_tem_con.py:19-54, model.py:358-372): img [N,D] image features of K clips stored clip after clip
+ * (clip_frames: HOST [K] frame counts summing to N), txt [P,D] text features, pairs: HOST [K][2] (source, target) text rows per clip.
+ * Writes img_norm [N], txt_norm [P] (L2 norms); logits [N][2] = scale * cos(frame, source|target), probs [N][2] their two-way softmax;
+ * success [N] int32 = logit_target >= logit_source; margin [N] = logit_target - logit_source; cosine [N] = cos(frame i, frame i+1) within
+ * the clip (NaN on a clip's last frame); clip_mean [K] = the mean of a clip's cosines (NaN for a one-frame clip). */
+int fz_clip_scores(const float* img, const float* txt, int N, int P, int D, const int* clip_frames, const int* pairs, int K, float scale,
+                   float* img_norm, float* txt_norm, float* logits, float* probs, int* success, float* margin, float* cosine, float* clip_mean,
+                   fz_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Frame-sharded execution over the GPUs of one NVSwitch box (one process per GPU): peer-memory exchange.
  * Replaces, for the frames-of-one-clip split of SURVEY.md §8(e), what the reference gets for free from holding every frame on one
  * device: K / V of other frames (prompt_attention/attention_register.py:162-193), joint-frame GroupNorm statistics
