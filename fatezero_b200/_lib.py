@@ -51,6 +51,11 @@ class AttnGroups(C.Structure):
     _fields_ = [("n_groups", c_int), ("g", AttnGroup * MAX_ATTN_GROUPS)]
 
 
+class AttnSlabs(C.Structure):
+    """fz_attn_slabs_t"""
+    _fields_ = [("store", c_void_p * MAX_ATTN_GROUPS), ("base", c_void_p * MAX_ATTN_GROUPS)]
+
+
 class P2PSeg(C.Structure):
     """fz_p2p_seg_t"""
     _fields_ = [("src", c_void_p), ("src_pitch", c_ll), ("dst", c_void_p), ("dst_pitch", c_ll), ("rows", c_int), ("row_bytes", c_int),
@@ -72,6 +77,7 @@ SIGNATURES = {
     "fz_tconv3_halo_f16": [c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p, c_int, C.POINTER(Epilogue), c_void_p, c_ll, c_int, c_void_p],
     "fz_attention_f16": [C.POINTER(AttnArgs), c_void_p],
     "fz_attention_grouped_f16": [C.POINTER(AttnArgs), C.POINTER(AttnGroups), c_void_p],
+    "fz_attention_grouped_slabs_f16": [C.POINTER(AttnArgs), C.POINTER(AttnGroups), C.POINTER(AttnSlabs), c_void_p],
     "fz_groupnorm_nhwc_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p,
                               c_void_p],
     "fz_groupnorm_batched_nhwc_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int,
@@ -92,6 +98,8 @@ SIGNATURES = {
     "fz_cfg_ddim_step": [c_void_p, c_void_p, c_ll, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p],
     "fz_cfg_ddim_step_batched": [c_void_p, c_void_p, c_int, c_ll, c_float, c_float, c_float, c_void_p, C.POINTER(c_void_p),
                                  C.POINTER(c_void_p), C.POINTER(c_int), c_ll, c_void_p],
+    "fz_cfg_ddim_step_multi": [c_void_p, c_void_p, c_int, c_ll, c_float, c_float, c_float, C.POINTER(c_void_p), C.POINTER(c_void_p),
+                               C.POINTER(c_void_p), C.POINTER(c_int), c_ll, c_void_p],
     "fz_blend_mask": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(c_float), c_float, c_int, c_int,
                       c_void_p, c_void_p],
     "fz_p2p_alloc": [c_ll, C.POINTER(c_void_p)],

@@ -293,6 +293,7 @@ class AttentionStore(AttentionControl):
             elif isinstance(v, dict):
                 v = {kk: (list(vv) if isinstance(vv, list) else vv) for kk, vv in v.items()}
             setattr(self, k, v)
+        self._self_sum_cache = None  # the replay refilled the slabs: a sum the template computed before it is stale
         self._graph_plan_id = getattr(tmpl, "_graph_plan_id", None)
 
     def reset(self):
@@ -677,6 +678,192 @@ class AttentionControlEditBatch:
             return
         for mine, theirs in zip(self.edits, tmpl.edits):
             mine.adopt_from(theirs)
+
+
+class AttentionStoreBatch:
+    """K inversion stores, one per source clip, filled by ONE batched inversion (UNet batch [clip_1..K], F frames each).
+
+    Every store is asked exactly what it is asked in its own batch-1 inversion (a LOW_RESOURCE batch of 1 at `frames` frames), so its slabs,
+    running sums, latents and step counter end up as `prepare_latents_ddim_inverted` leaves `pipe.store_controller`; the answers are merged
+    into one grouped launch (fz_attention_grouped_slabs_f16: clip k owns rows [k F, (k + 1) F) and writes its own slabs).
+    store_maps=False: no maps are stored (prepare_latents_ddim_inverted with store_attention=False); the stores still record the latents,
+    and the batch still makes the UNet plan its GroupNorm statistics per clip."""
+
+    def __init__(self, stores: List[AttentionStore], store_maps: bool = True):
+        stores = list(stores)
+        if not stores or len(stores) > _lib.MAX_ATTN_GROUPS:
+            raise ValueError(f"AttentionStoreBatch: 1..{_lib.MAX_ATTN_GROUPS} stores, got {len(stores)}")
+        if any(not isinstance(s, AttentionStore) or isinstance(s, AttentionControlEdit) for s in stores):
+            raise TypeError("AttentionStoreBatch: every clip needs its own AttentionStore")
+        if len({id(s) for s in stores}) != len(stores):
+            raise ValueError("AttentionStoreBatch: a store appears twice (one store per clip)")
+        if any(s.disk_store or s.host_spill for s in stores):
+            raise NotImplementedError("AttentionStoreBatch: disk_store / host_spill stores are inverted one clip at a time")
+        if len({bool(s.save_self_attention) for s in stores}) != 1:
+            raise ValueError("AttentionStoreBatch: the stores disagree on save_self_attention")
+        self.stores = stores
+        self.store_maps = bool(store_maps)
+        self.prompt_groups = len(stores)
+        self.num_att_layers = -1
+
+    def __setattr__(self, name, value):
+        object.__setattr__(self, name, value)
+        if name == "num_att_layers":
+            for s in self.__dict__.get("stores", []):
+                s.num_att_layers = value
+
+    @property
+    def cur_step(self) -> int:
+        return self.stores[0].cur_step
+
+    # ---- fused-kernel protocol ------------------------------------------------------------------------------------------
+    def begin_forward(self, batch, frames):
+        if batch != self.prompt_groups:
+            raise RuntimeError(f"AttentionStoreBatch: expected a batch of {self.prompt_groups} clips, got {batch}")
+        for s in self.stores:
+            s.begin_forward(1, frames)
+
+    def _merge(self, answers: List[Optional[dict]]) -> Optional[dict]:
+        if self.prompt_groups == 1:
+            return answers[0]
+        if all(a is None for a in answers):
+            return None
+        if any(a is None or a["edit_bf_start"] != 0 for a in answers):
+            raise RuntimeError("AttentionStoreBatch: every clip must store all of its rows (LOW_RESOURCE inversion)")
+        return dict(edit_bf_start=0, cache_ld=answers[0]["cache_ld"],
+                    groups=[dict(row_mode=_lib.ATTN_STORE, store=a["store"], acc=a.get("acc")) for a in answers])
+
+    def self_attn_args(self, place, S, T, heads, nb, frames):
+        if not self.store_maps:
+            return None
+        return self._merge([s.self_attn_args(place, S, T, heads, frames, frames) for s in self.stores])
+
+    def cross_attn_args(self, place, S, heads, nb, frames):
+        if not self.store_maps:
+            return None
+        return self._merge([s.cross_attn_args(place, S, heads, frames, frames) for s in self.stores])
+
+    def step_callback(self, x_t):
+        for k, s in enumerate(self.stores):
+            s.step_callback(x_t[k:k + 1])
+        return x_t
+
+    def reset(self):
+        for s in self.stores:
+            s.reset()
+
+    # ---- CUDA-graph replay support (graphs.py), composed from the stores' --------------------------------------------------
+    def graph_signature(self):
+        sigs = [s.graph_signature() for s in self.stores]
+        if any(s is None for s in sigs):
+            return None
+        return ("store_batch", len(sigs), self.store_maps, sigs[0])
+
+    def is_pristine(self) -> bool:
+        return all(s.is_pristine() for s in self.stores)
+
+    @property
+    def _graph_plan_id(self):
+        return tuple(s._graph_plan_id for s in self.stores)
+
+    @_graph_plan_id.setter
+    def _graph_plan_id(self, plan_id):
+        # clip k's maps are its own slabs of the plan: (plan, k) tells them apart in the key of a captured edit that reads them
+        for k, s in enumerate(self.stores):
+            s._graph_plan_id = (plan_id, k)
+
+    def adopt_from(self, tmpl: "AttentionStoreBatch"):
+        if tmpl is self:
+            return
+        for mine, theirs in zip(self.stores, tmpl.stores):
+            mine.adopt_from(theirs)
+
+
+class AttentionControlEditClips(AttentionControlEditBatch):
+    """K edit controllers of possibly DIFFERENT inverted clips driven through one batched edit pass (CFG batch [uncond_1..K ; cond_1..K]).
+
+    As AttentionControlEditBatch, each child is asked what its own single-prompt pass asks, but every group reads the cached maps of its
+    own child's additional_attention_store (fz_attention_grouped_slabs_f16), and the latent blend of each child uses its own store's
+    inverted latents (fz_cfg_ddim_step_multi).  Several children may edit the same clip."""
+
+    def __init__(self, edits: List[AttentionControlEdit]):
+        edits = list(edits)
+        if not edits or len(edits) > _lib.MAX_ATTN_GROUPS:
+            raise ValueError(f"AttentionControlEditClips: 1..{_lib.MAX_ATTN_GROUPS} edit controllers, got {len(edits)}")
+        c0 = edits[0]
+        for e in edits[1:]:
+            if e.num_steps != c0.num_steps or bool(e.use_inversion_attention) != bool(c0.use_inversion_attention):
+                raise ValueError("AttentionControlEditClips: every edit must share num_steps and use_inversion_attention")
+        for e in edits:
+            st = e.additional_attention_store
+            if getattr(e, "disk_store", False) or getattr(st, "disk_store", False) or getattr(st, "host_spill", False):
+                raise NotImplementedError("AttentionControlEditClips: disk_store / host_spill stores are edited one clip at a time")
+        self.edits = edits
+        self.prompt_groups = len(edits)
+        self.LOW_RESOURCE = False
+        self.num_att_layers = -1
+        self._frames = None
+
+    @property
+    def additional_attention_store(self):
+        raise AttributeError("AttentionControlEditClips: every edit has its own additional_attention_store (see .edits)")
+
+    def _merge(self, answers: List[Optional[dict]], frames: int) -> Optional[dict]:
+        if self.prompt_groups == 1:
+            return answers[0]
+        live = [a for a in answers if a is not None]
+        if not live:
+            return None
+        cache_ld = live[0]["cache_ld"]
+        for a in live:
+            if a["cache_ld"] != cache_ld or a["base"].shape != live[0]["base"].shape:
+                raise RuntimeError("AttentionControlEditClips: the clips' cached inversion maps of this layer differ in geometry")
+            if a["edit_bf_start"] != frames:
+                raise RuntimeError("AttentionControlEditClips: an edit asked for rows outside its conditional half")
+        groups = [dict(row_mode=_lib.ATTN_NONE) if a is None else
+                  dict(row_mode=a["row_mode"], mask=a.get("mask"), acc=a.get("acc"), xedit=a.get("xedit"), base=a["base"]) for a in answers]
+        return dict(edit_bf_start=self.prompt_groups * frames, cache_ld=cache_ld, groups=groups)
+
+    def graph_signature(self):
+        sigs = [e.graph_signature() for e in self.edits]
+        if any(s is None for s in sigs):
+            return None
+        # which store each child reads is part of the launch sequence (the base slabs are baked into the captured kernels); the last
+        # element lists the stores' plan ids, None when one of them does not live in a captured inversion plan
+        plans = tuple(s[-1] for s in sigs)
+        stores = [id(e.additional_attention_store) for e in self.edits]
+        layout = tuple(stores.index(s) for s in stores)
+        return ("edit_clips", tuple(s[:-1] for s in sigs), layout, None if any(p is None for p in plans) else plans)
+
+
+def map_cache_bytes(unet_config: dict, model_config: dict, h: int, w: int, save_self_attention: bool = True) -> Tuple[int, int]:
+    """HBM of one clip frame's inversion map cache at latent size h x w: (bytes per DDIM step, bytes held once: the cross running sums).
+    Restates the slab shapes AttentionStore allocates for the UNet's transformer layers (self maps [heads, S, n_slots S], cross maps
+    [heads, S, 80] and their sums, for S <= 32^2) so that a batch can be admitted before any of it is allocated."""
+    ch = list(unet_config["block_out_channels"])
+    heads = int(unet_config["attention_head_dim"])
+    lpb = int(unet_config["layers_per_block"])
+    nblk = len(ch)
+    layers = []  # (channels, S)
+    for i, t in enumerate(unet_config["down_block_types"]):
+        if t.startswith("CrossAttn"):
+            layers += [(ch[i], (h >> i) * (w >> i))] * lpb
+    layers.append((ch[-1], (h >> (nblk - 1)) * (w >> (nblk - 1))))
+    for i, t in enumerate(unet_config["up_block_types"]):
+        if t.startswith("CrossAttn"):
+            s = nblk - 1 - i
+            layers += [(ch[s], (h >> s) * (w >> s))] * (lpb + 1)
+    index_list = list(model_config.get("SparseCausalAttention_index", [-1, "first"]))
+    per_step = once = 0
+    for c, S in layers:
+        if S > 32 ** 2:
+            continue
+        slots = len(index_list) if index_list and not ("least_sc_channel" in model_config and c < model_config["least_sc_channel"]) else 1
+        if save_self_attention:
+            per_step += heads * S * slots * S * 2
+        per_step += heads * S * CROSS_LD * 2
+        once += heads * S * CROSS_LD * 2
+    return per_step, once
 
 
 def get_equalizer(text: str, word_select, values, tokenizer=None):

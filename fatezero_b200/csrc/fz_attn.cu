@@ -12,7 +12,8 @@
 //   BLEND      edit, self-attention with a per-(frame,pixel) mask: rows with mask==0 take the cached row (:86-88)
 //   CROSSEDIT  edit, cross-attention: Refine gather / Replace 77x77 / Reweight / alpha-lerp in registers (:130-131,213-253,282-286)
 // The hook is chosen per row group (fz_attention_grouped_f16: K prompts of one clip in one CFG batch, each group with its own mode, mask,
-// running sum and edit tables, all reading one cached map); fz_attention_f16 is the one-group case.
+// running sum and edit tables; fz_attention_grouped_slabs_f16: groups of different clips, each with its own cache slab to store into or
+// read from); fz_attention_f16 is the one-group case.
 // Hooked rows take two passes over the keys (max and sum first, then probabilities): the normalised fp16 P the reference stores and
 // multiplies is reproduced exactly at its rounding point.  Rows that are neither stored nor edited take ONE pass with a running reference
 // maximum (online softmax: p = exp2(s c - m_ref c) rounded to fp16 for PV, fp32 row sum l, O / l at the end; m_ref is raised, and O, l
@@ -44,8 +45,9 @@ struct AttnParams {
   CUtensorMap tmQ;      // (d, heads, S_q, BF)                 box (64, 1, 128, 1)
   CUtensorMap tmK;      // (d, heads, keys_per_slot, SRC)      box (64, 1, 64, 1)
   CUtensorMap tmVt;     // (keys_ld, d, heads, SRC)            box (64, 64 nd, 1, 1)
-  CUtensorMap tmStore;  // (keys_ld_cache, slots, S_q, heads, Fc) box (64, 1, 64, 1, 1)   cache slab written (STORE)
-  CUtensorMap tmBase;   // same geometry, cache slab read (REPLACE / BLEND)
+  // per group: the cache slab it writes (STORE) or reads (REPLACE / BLEND), (keys_ld_cache, slots, S_q, heads, Fc) box (64, 1, 64, 1, 1);
+  // a group is never both, so one map per group
+  CUtensorMap tmCache[FZ_ATTN_MAX_GROUPS];
   int S_q;              // queries per (frame, head)
   int keys_per_slot;    // S for self-attention, 77 for cross
   int n_slots;          // key/value frames per query frame (self: 1..4, cross: 1)
@@ -55,7 +57,7 @@ struct AttnParams {
   float scale_log2;     // scale * log2(e)
   int src_index[kMaxSlots][kMaxBFGrouped];  // K/V source row (frame or text batch) per slot and query frame
   // controller: rows bf >= edit_bf_start form n_groups groups of group_rows rows; row bf belongs to group
-  // g = (bf - edit_bf_start) / group_rows and reads cache frame fc = (bf - edit_bf_start) % group_rows of the shared base slab
+  // g = (bf - edit_bf_start) / group_rows and stores / reads cache frame fc = (bf - edit_bf_start) % group_rows of its slab
   int edit_bf_start;
   int group_rows;       // Fc: rows per group (the base / store slabs are [Fc, heads, S_q, cache_ld])
   int n_groups;
@@ -66,7 +68,7 @@ struct AttnParams {
   const float* g_xedit[kMaxGroups];  // CROSSEDIT tables in device memory (fz_cross_edit_t layout), per group
   const float* g_mask[kMaxGroups];   // BLEND: [Fc, S_q] 1 = keep current row, 0 = take cached row, per group
   long long acc_ld;
-  const __half* base_rows;  // CROSSEDIT: cached source map [Fc, heads, S_q, base_ld]
+  const __half* g_base_rows[FZ_ATTN_MAX_GROUPS];  // CROSSEDIT: cached source map [Fc, heads, S_q, base_ld], per group
   long long base_ld;
   __half* out;          // [BF*S_q, ldo], this head's columns start at head*d
   long long ldo;
@@ -202,7 +204,7 @@ __global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ At
         mbar_wait(&base_empty[b], ((A >> 1) & 1) ^ 1);
         mbar_expect_tx(&base_full[b], kAtomBytes);
         for (int h = 0; h < 2; ++h)
-          tma_load_5d(s_base + b * kAtomBytes + h * kHalfAtom, &p.tmBase, &base_full[b], ai.k0, ai.slot, q0 + 64 * h, head, fc);
+          tma_load_5d(s_base + b * kAtomBytes + h * kHalfAtom, &p.tmCache[grp], &base_full[b], ai.k0, ai.slot, q0 + 64 * h, head, fc);
       };
       if (!replace) {
         mbar_expect_tx(q_full, p.nd * kAtomBytes);
@@ -366,7 +368,7 @@ __global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ At
             }
           }
           if (row_mode == FZ_ATTN_CROSSEDIT) {
-            const __half* brow = p.base_rows + rbase * p.base_ld;
+            const __half* brow = p.g_base_rows[grp] + rbase * p.base_ld;
             const float* xe = p.g_xedit[grp];
             const int xmode = static_cast<int>(xe[0]);  // 0 refine, 1 replace
             const float* x_alpha = xe + 8;              // [80] cross_replace_alpha of this step
@@ -447,7 +449,7 @@ __global__ void __launch_bounds__(288, 1) attn_kernel(const __grid_constant__ At
       fence_proxy_async_smem();
       named_bar_sync(1 + wg, 128);
       if (row_mode == FZ_ATTN_STORE && st == 0) {
-        tma_store_5d(&p.tmStore, ptile, ai.k0, ai.slot, q0 + 64 * wg, head, fc);
+        tma_store_5d(&p.tmCache[grp], ptile, ai.k0, ai.slot, q0 + 64 * wg, head, fc);
         tma_store_commit();
       }
       mbar_wait(&ring_full[stage], phase);
@@ -499,9 +501,11 @@ static int encode_cache_map(CUtensorMap* tm, const void* base, int keys_ld_slot,
   return encode_tmap_f16(tm, base, 5, dims, strides, box, true);
 }
 
-// One launcher for both entries.  `g` carries the controller hook per row group; rows [edit_bf_start, BF) form g->n_groups groups of
-// group_rows rows, all reading the same base slab [group_rows, heads, S_q, cache_ld].
-static int attention_launch(const fz_attn_args_t* a, const fz_attn_groups_t* g, int group_rows, cudaStream_t stream) {
+// One launcher for every entry.  `g` carries the controller hook per row group; rows [edit_bf_start, BF) form g->n_groups groups of
+// group_rows rows.  Group k stores into / reads the slab [group_rows, heads, S_q, cache_ld] slabs->store[k] / slabs->base[k], or the slab
+// of `a` where that is NULL (slabs == NULL: every group uses the slabs of `a`).
+static int attention_launch(const fz_attn_args_t* a, const fz_attn_groups_t* g, const fz_attn_slabs_t* slabs, int group_rows,
+                            cudaStream_t stream) {
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.S_q = a->S_q; p.keys_per_slot = a->keys_per_slot; p.n_slots = a->n_slots;
@@ -514,17 +518,24 @@ static int attention_launch(const fz_attn_args_t* a, const fz_attn_groups_t* g, 
   p.group_rows = std::max(1, group_rows);
   p.n_groups = g->n_groups;
   for (int i = std::max(0, a->edit_bf_start); i < a->BF; ++i) p.row_group[i] = static_cast<unsigned char>((i - a->edit_bf_start) / p.group_rows);
-  bool any_store = false, any_base = false, any_self_base = false, any_hook = false;
+  bool any_slab = false, any_self_base = false, any_hook = false;
+  const void* store_of[kMaxGroups];
+  const void* base_of[kMaxGroups];
   for (int k = 0; k < g->n_groups; ++k) {
     const fz_attn_group_t& gr = g->g[k];
+    store_of[k] = slabs && slabs->store[k] ? slabs->store[k] : a->store;
+    base_of[k] = slabs && slabs->base[k] ? slabs->base[k] : a->base;
     FZ_CHECK_ARG(gr.row_mode >= FZ_ATTN_NONE && gr.row_mode <= FZ_ATTN_CROSSEDIT, "fz_attention: group %d: row_mode %d unknown", k, gr.row_mode);
     p.g_row_mode[k] = gr.row_mode;
     p.g_acc[k] = static_cast<__half*>(gr.acc);
     p.g_xedit[k] = gr.xedit;
     p.g_mask[k] = gr.mask;
-    any_store |= gr.row_mode == FZ_ATTN_STORE;
+    p.g_base_rows[k] = static_cast<const __half*>(base_of[k]);
+    const bool reads_base = gr.row_mode == FZ_ATTN_REPLACE || gr.row_mode == FZ_ATTN_BLEND || gr.row_mode == FZ_ATTN_CROSSEDIT;
+    if (gr.row_mode == FZ_ATTN_STORE) FZ_CHECK_ARG(store_of[k], "fz_attention: STORE needs a cache slab (group %d)", k);
+    if (reads_base) FZ_CHECK_ARG(base_of[k], "fz_attention: REPLACE/BLEND/CROSSEDIT need the cached source map (group %d)", k);
+    any_slab |= store_of[k] != nullptr || base_of[k] != nullptr;
     any_self_base |= gr.row_mode == FZ_ATTN_REPLACE || gr.row_mode == FZ_ATTN_BLEND;
-    any_base |= gr.row_mode == FZ_ATTN_REPLACE || gr.row_mode == FZ_ATTN_BLEND || gr.row_mode == FZ_ATTN_CROSSEDIT;
     any_hook |= gr.row_mode != FZ_ATTN_NONE || gr.acc != nullptr;
     if (gr.row_mode == FZ_ATTN_BLEND) FZ_CHECK_ARG(gr.mask, "fz_attention: BLEND needs a mask");
     if (gr.row_mode == FZ_ATTN_CROSSEDIT) FZ_CHECK_ARG(gr.xedit && a->n_slots == 1 && a->keys_per_slot <= 80, "fz_attention: CROSSEDIT needs tables, one slot, <= 80 keys");
@@ -532,15 +543,13 @@ static int attention_launch(const fz_attn_args_t* a, const fz_attn_groups_t* g, 
   }
   p.has_base = any_self_base;
   p.acc_ld = a->acc_ld;
-  p.base_rows = static_cast<const __half*>(a->base); p.base_ld = a->cache_ld;
+  p.base_ld = a->cache_ld;
   p.out = static_cast<__half*>(a->out); p.ldo = a->ldo;
   p.causal = a->causal;
   p.masked = a->causal || a->keys_per_slot % 64 != 0;
   if (a->causal) FZ_CHECK_ARG(a->n_slots == 1 && !any_hook, "fz_attention: causal masking needs one slot and no controller hook");
   const int Fc = group_rows;
-  if (any_store) FZ_CHECK_ARG(a->store, "fz_attention: STORE needs a cache slab");
-  if (any_base) FZ_CHECK_ARG(a->base, "fz_attention: REPLACE/BLEND/CROSSEDIT need the cached source map");
-  if (a->store || a->base)
+  if (any_slab || a->store || a->base)
     FZ_CHECK_ARG(a->cache_ld > 0 && a->cache_ld % a->n_slots == 0 && a->cache_ld / a->n_slots >= a->keys_per_slot,
                  "fz_attention: cache_ld=%lld must split into n_slots=%d runs of >= keys_per_slot=%d keys", a->cache_ld, a->n_slots,
                  a->keys_per_slot);
@@ -562,16 +571,24 @@ static int attention_launch(const fz_attn_args_t* a, const fz_attn_groups_t* g, 
     uint32_t box[4] = {64, (uint32_t)(64 * p.nd), 1, 1};  // rows beyond d: zero fill (fixed-shape PV wgmma)
     if (int rc = encode_tmap_f16(&p.tmVt, a->vt, 4, dims, strides, box, true)) return rc;
   }
-  // cache geometry: a row of the slab is n_slots * keys_ld_slot wide, keys_ld_slot = cache_ld / n_slots
-  if (a->store) {
-    if (int rc = encode_cache_map(&p.tmStore, a->store, (int)(a->cache_ld / a->n_slots), a->n_slots, a->S_q, a->heads, Fc, a->cache_ld)) return rc;
-  } else {
-    p.tmStore = p.tmQ;
-  }
-  if (a->base && any_self_base) {
-    if (int rc = encode_cache_map(&p.tmBase, a->base, (int)(a->cache_ld / a->n_slots), a->n_slots, a->S_q, a->heads, Fc, a->cache_ld)) return rc;
-  } else {
-    p.tmBase = p.tmQ;
+  // cache geometry: a row of the slab is n_slots * keys_ld_slot wide, keys_ld_slot = cache_ld / n_slots.  Groups that share a slab share
+  // its encoded map; groups without a TMA-accessed slab (NONE, CROSSEDIT) get a placeholder that is never used.
+  for (int k = 0; k < kMaxGroups; ++k) {
+    const int mode = k < g->n_groups ? g->g[k].row_mode : FZ_ATTN_NONE;
+    const void* slab = mode == FZ_ATTN_STORE ? store_of[k] : (mode == FZ_ATTN_REPLACE || mode == FZ_ATTN_BLEND) ? base_of[k] : nullptr;
+    int same = -1;
+    for (int j = 0; j < k && slab; ++j) {
+      const int mj = g->g[j].row_mode;
+      const void* sj = mj == FZ_ATTN_STORE ? store_of[j] : (mj == FZ_ATTN_REPLACE || mj == FZ_ATTN_BLEND) ? base_of[j] : nullptr;
+      if (sj == slab) { same = j; break; }
+    }
+    if (!slab) {
+      p.tmCache[k] = p.tmQ;
+    } else if (same >= 0) {
+      p.tmCache[k] = p.tmCache[same];
+    } else if (int rc = encode_cache_map(&p.tmCache[k], slab, (int)(a->cache_ld / a->n_slots), a->n_slots, a->S_q, a->heads, Fc, a->cache_ld)) {
+      return rc;
+    }
   }
   // shared memory plan: Q + ring + 4 half P tiles (+ 2 base tiles) + barriers
   const int stage_bytes = p.nd * 64 * 128;
@@ -614,16 +631,19 @@ extern "C" int fz_attention_f16(const fz_attn_args_t* a, cudaStream_t stream) {
   g.g[0].xedit = a->xedit;
   g.g[0].mask = a->mask;
   g.g[0].acc = a->acc;
-  return attention_launch(a, &g, a->BF - a->edit_bf_start, stream);
+  return attention_launch(a, &g, nullptr, a->BF - a->edit_bf_start, stream);
 }
 
-extern "C" int fz_attention_grouped_f16(const fz_attn_args_t* a, const fz_attn_groups_t* g, cudaStream_t stream) {
+extern "C" int fz_attention_grouped_slabs_f16(const fz_attn_args_t* a, const fz_attn_groups_t* g, const fz_attn_slabs_t* slabs,
+                                              cudaStream_t stream) {
   if (int rc = check_common(a, kMaxBFGrouped)) return rc;
   FZ_CHECK_ARG(g && g->n_groups >= 1 && g->n_groups <= kMaxGroups, "fz_attention_grouped: n_groups=%d unsupported (1..%d)", g ? g->n_groups : 0,
                kMaxGroups);
   FZ_CHECK_ARG(a->F >= 1 && a->edit_bf_start >= 0 && a->BF - a->edit_bf_start == g->n_groups * a->F,
                "fz_attention_grouped: BF - edit_bf_start = %d rows must be n_groups * F = %d * %d", a->BF - a->edit_bf_start, g->n_groups, a->F);
-  for (int k = 0; k < g->n_groups; ++k)
-    FZ_CHECK_ARG(g->g[k].row_mode != FZ_ATTN_STORE, "fz_attention_grouped: group %d: STORE is not a grouped mode", k);
-  return attention_launch(a, g, a->F, stream);
+  return attention_launch(a, g, slabs, a->F, stream);
+}
+
+extern "C" int fz_attention_grouped_f16(const fz_attn_args_t* a, const fz_attn_groups_t* g, cudaStream_t stream) {
+  return fz_attention_grouped_slabs_f16(a, g, nullptr, stream);
 }

@@ -662,17 +662,18 @@ __global__ void ddim_invert_kernel(float* __restrict__ x, const float* __restric
 }
 
 // K items of n_item elements: x [K, n_item], eps2 = [uncond_1..K | cond_1..K]. mask (optional, per item): [F*H*W] floats per frame pixel,
-// broadcast over channels; x_inv [n_item] is shared by the items.
+// broadcast over channels; x_inv (per item, [n_item]): the inverted latent the item blends towards (items of one clip share it).
 constexpr int kCfgMaxItems = 8;
 struct CfgItems {
+  const float* x_inv[kCfgMaxItems];
   const float* mask_a[kCfgMaxItems];
   const float* mask_b[kCfgMaxItems];
   int apply_blend[kCfgMaxItems];
 };
 
 __global__ void cfg_ddim_kernel(float* __restrict__ x, const float* __restrict__ eps2, int K, long long n_item, float guidance, float sqrt_a_t,
-                                float sqrt_1m_a_t, float sqrt_a_prev, float sqrt_1m_a_prev, const float* __restrict__ x_inv,
-                                const __grid_constant__ CfgItems items, long long fhw) {
+                                float sqrt_1m_a_t, float sqrt_a_prev, float sqrt_1m_a_prev, const __grid_constant__ CfgItems items,
+                                long long fhw) {
   const long long n = static_cast<long long>(K) * n_item;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float eu = eps2[i], ec = eps2[n + i];
@@ -685,7 +686,7 @@ __global__ void cfg_ddim_kernel(float* __restrict__ x, const float* __restrict__
       const long long q = j % fhw;
       float m = items.mask_a[k][q];
       if (items.mask_b[k]) m = fmaxf(m, items.mask_b[k][q]);
-      const float xi = x_inv[j];
+      const float xi = items.x_inv[k][j];
       xn = xi + m * (xn - xi);
     }
     x[i] = xn;
@@ -986,10 +987,10 @@ extern "C" int fz_ddim_invert_step(float* x, const float* eps, long long n, floa
   return FZ_OK;
 }
 
-static int cfg_ddim_launch(float* x, const float* eps2, int K, long long n_item, float guidance, float a_t, float a_prev, const float* x_inv,
-                           const CfgItems& items, long long fhw, cudaStream_t stream) {
+static int cfg_ddim_launch(float* x, const float* eps2, int K, long long n_item, float guidance, float a_t, float a_prev, const CfgItems& items,
+                           long long fhw, cudaStream_t stream) {
   cfg_ddim_kernel<<<grid_for(static_cast<long long>(K) * n_item, 256), 256, 0, stream>>>(
-      x, eps2, K, n_item, guidance, sqrtf(a_t), sqrtf(1.f - a_t), sqrtf(a_prev), sqrtf(1.f - a_prev), x_inv, items, fhw);
+      x, eps2, K, n_item, guidance, sqrtf(a_t), sqrtf(1.f - a_t), sqrtf(a_prev), sqrtf(1.f - a_prev), items, fhw);
   FZ_CUDA(cudaGetLastError());
   return FZ_OK;
 }
@@ -1003,7 +1004,8 @@ extern "C" int fz_cfg_ddim_step(float* x, const float* eps2, long long n, float 
   items.mask_a[0] = mask_a;
   items.mask_b[0] = mask_b;
   items.apply_blend[0] = apply_blend;
-  return cfg_ddim_launch(x, eps2, 1, n, guidance, a_t, a_prev, x_inv, items, fhw, stream);
+  items.x_inv[0] = x_inv;
+  return cfg_ddim_launch(x, eps2, 1, n, guidance, a_t, a_prev, items, fhw, stream);
 }
 
 extern "C" int fz_cfg_ddim_step_batched(float* x, const float* eps2, int K, long long n_item, float guidance, float a_t, float a_prev,
@@ -1017,9 +1019,28 @@ extern "C" int fz_cfg_ddim_step_batched(float* x, const float* eps2, int K, long
     items.mask_a[k] = mask_a ? mask_a[k] : nullptr;
     items.mask_b[k] = mask_b ? mask_b[k] : nullptr;
     items.apply_blend[k] = apply_blend ? apply_blend[k] : 0;
+    items.x_inv[k] = x_inv;
     FZ_CHECK_ARG(!items.apply_blend[k] || (x_inv && items.mask_a[k] && fhw > 0), "fz_cfg_ddim_step_batched: item %d: blend needs x_inv and mask", k);
   }
-  return cfg_ddim_launch(x, eps2, K, n_item, guidance, a_t, a_prev, x_inv, items, fhw, stream);
+  return cfg_ddim_launch(x, eps2, K, n_item, guidance, a_t, a_prev, items, fhw, stream);
+}
+
+extern "C" int fz_cfg_ddim_step_multi(float* x, const float* eps2, int K, long long n_item, float guidance, float a_t, float a_prev,
+                                      const float* const* x_inv, const float* const* mask_a, const float* const* mask_b, const int* apply_blend,
+                                      long long fhw, cudaStream_t stream) {
+  FZ_CHECK_ARG(x && eps2 && n_item > 0, "fz_cfg_ddim_step_multi: null pointer");
+  FZ_CHECK_ARG(K >= 1 && K <= kCfgMaxItems, "fz_cfg_ddim_step_multi: K=%d unsupported (1..%d)", K, kCfgMaxItems);
+  CfgItems items;
+  memset(&items, 0, sizeof(items));
+  for (int k = 0; k < K; ++k) {
+    items.x_inv[k] = x_inv ? x_inv[k] : nullptr;
+    items.mask_a[k] = mask_a ? mask_a[k] : nullptr;
+    items.mask_b[k] = mask_b ? mask_b[k] : nullptr;
+    items.apply_blend[k] = apply_blend ? apply_blend[k] : 0;
+    FZ_CHECK_ARG(!items.apply_blend[k] || (items.x_inv[k] && items.mask_a[k] && fhw > 0), "fz_cfg_ddim_step_multi: item %d: blend needs x_inv and mask",
+                 k);
+  }
+  return cfg_ddim_launch(x, eps2, K, n_item, guidance, a_t, a_prev, items, fhw, stream);
 }
 
 extern "C" int fz_blend_mask(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int r, int ldm, int ntok, const float* word_w,

@@ -271,6 +271,22 @@ def cfg_ddim_step_batched(x: torch.Tensor, eps2: torch.Tensor, guidance: float, 
               fhw, _stream())
 
 
+def cfg_ddim_step_multi(x: torch.Tensor, eps2: torch.Tensor, guidance: float, a_t: float, a_prev: float,
+                        blends: Optional[Sequence[Optional[dict]]] = None):
+    """x [K, 4, F, h, w] fp32 (K items, possibly of different clips), eps2 [2K, ...] = [uncond_1..K ; cond_1..K]; blends: one
+    latent_blend_args() dict (or None) per item, each with the x_inv of its own clip."""
+    K = x.shape[0]
+    fhw = x.shape[-3] * x.shape[-2] * x.shape[-1]
+    blends = list(blends) if blends is not None else [None] * K
+    assert len(blends) == K and eps2.shape[0] == 2 * K
+    xi = (C.c_void_p * K)(*[None if b is None else b["x_inv"].data_ptr() for b in blends])
+    ma = (C.c_void_p * K)(*[None if b is None else b["mask_a"].data_ptr() for b in blends])
+    mb = (C.c_void_p * K)(*[None if b is None or b["mask_b"] is None else b["mask_b"].data_ptr() for b in blends])
+    ap = (C.c_int * K)(*[int(b is not None and bool(b["apply_blend"])) for b in blends])
+    _lib.call("fz_cfg_ddim_step_multi", _p(x), _p(eps2), K, x.numel() // K, float(guidance), float(a_t), float(a_prev), xi, ma, mb, ap, fhw,
+              _stream())
+
+
 def blend_mask(maps: Sequence[torch.Tensor], word_w: torch.Tensor, th: float, h: int, w: int) -> torch.Tensor:
     """maps: list of [F, heads, r*r, ld] (fp16 cache slabs or fp16 running sums) -> mask [F, h, w] float 0/1."""
     m0 = maps[0]
@@ -403,8 +419,9 @@ def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, out: torch.Ten
               row_mode: int = _lib.ATTN_NONE, store=None, base=None, cache_ld: int = 0, acc=None, xedit=None, mask=None, dbg=None,
               causal: bool = False, groups: Optional[Sequence[dict]] = None):
     """q/k: strided 2-D views (rows, ld) whose column h*d starts head h; vt [n_src, heads, d, vt_ld]; out [BF*S_q, ldo].
-    groups (batched edits): one dict(row_mode=, mask=, acc=, xedit=) per edited row group of F rows after edit_bf_start, all reading `base`;
-    row_mode / acc / xedit / mask must then be left at their defaults."""
+    groups (batched edits and inversions): one dict(row_mode=, mask=, acc=, xedit=, store=, base=) per row group of F rows after
+    edit_bf_start; a group without `store` / `base` uses the slab given here.  row_mode / acc / xedit / mask must then be left at their
+    defaults."""
     a = AttnArgs()
     a.q, a.ldq = _p(q), q.stride(0)
     a.k, a.ldk = _p(k), k.stride(0)
@@ -436,5 +453,11 @@ def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, out: torch.Ten
         gs.g[i].xedit, gs.g[i].mask, gs.g[i].acc = _p(g.get("xedit")), _p(g.get("mask")), _p(g.get("acc"))
         if g.get("acc") is not None:
             a.acc_ld = g["acc"].stride(2)
-    _lib.call("fz_attention_grouped_f16", C.byref(a), C.byref(gs), _stream())
+    if all(g.get("store") is None and g.get("base") is None for g in groups):
+        _lib.call("fz_attention_grouped_f16", C.byref(a), C.byref(gs), _stream())
+        return out
+    sl = _lib.AttnSlabs()
+    for i, g in enumerate(groups):
+        sl.store[i], sl.base[i] = _p(g.get("store")), _p(g.get("base"))
+    _lib.call("fz_attention_grouped_slabs_f16", C.byref(a), C.byref(gs), C.byref(sl), _stream())
     return out

@@ -341,7 +341,8 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
 
             # ---- CUDA-graph path (graphs.py): same launch sequence, captured once per configuration, no Python in the step ----
             sig = None
-            if (self.graph_mode != "off" and teacher_latents is None and isinstance(controller, attention_util.AttentionStore)
+            if (self.graph_mode != "off" and teacher_latents is None
+                    and isinstance(controller, (attention_util.AttentionStore, attention_util.AttentionStoreBatch))
                     and getattr(self.unet, "_controller", None) is controller and controller.is_pristine()):
                 sig = controller.graph_signature()
             key = None if sig is None else ("inv", tuple(latent.shape), str(weight_dtype), tuple(ts), tuple(cond.shape), sig,
@@ -391,8 +392,9 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         return self.scheduler.timesteps[t_start:], num_inference_steps - t_start
 
     # ---- edit -----------------------------------------------------------------------------------------------------------
-    def _make_edit_controller(self, prompt: str, source_prompt: str, num_inference_steps: int, **kwargs):
-        """The make_controller call of p2p_ddim_spatial_temporal.py:176-193: one target prompt against the inversion store."""
+    def _make_edit_controller(self, prompt: str, source_prompt: str, num_inference_steps: int, store=None, **kwargs):
+        """The make_controller call of p2p_ddim_spatial_temporal.py:176-193: one target prompt against the inversion store (`store`, by
+        default self.store_controller)."""
         len_source = len(source_prompt.split(" "))
         len_target = len(prompt.split(" "))
         equal_length = len_source == len_target
@@ -401,7 +403,8 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
             is_replace_controller=kwargs.get("is_replace_controller", True) and equal_length,
             cross_replace_steps=kwargs["cross_replace_steps"], self_replace_steps=kwargs["self_replace_steps"],
             blend_words=kwargs.get("blend_words", None), equilizer_params=kwargs.get("eq_params", None),
-            additional_attention_store=self.store_controller, use_inversion_attention=kwargs["use_inversion_attention"],
+            additional_attention_store=self.store_controller if store is None else store,
+            use_inversion_attention=kwargs["use_inversion_attention"],
             blend_th=kwargs.get("blend_th", (0.3, 0.3)), blend_self_attention=kwargs.get("blend_self_attention", None),
             blend_latents=kwargs.get("blend_latents", None), save_path=kwargs.get("save_path", None),
             save_self_attention=kwargs.get("save_self_attention", True), disk_store=kwargs.get("disk_store", False))
@@ -468,7 +471,11 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
                                         callback_steps=callback_steps, controller=batch)
         finally:
             attention_util.register_attention_control(self, self.empty_controller)
-        lat = out.images
+        self.last_edit_controllers = edits
+        return self._batch_results(prompts, edits, out.images, output_type)
+
+    def _batch_results(self, prompts, edits, lat, output_type):
+        """One p2preplace_edit result dict per prompt of a batched edit."""
         results = []
         for k, (pr, e) in enumerate(zip(prompts, edits)):
             lk = lat[k:k + 1]
@@ -483,8 +490,167 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
                 from .visualization import show_cross_attention
                 attention_output = show_cross_attention(self.tokenizer, pr, e, 16, ["up", "down"])
             results.append({"sdimage_output": sd, "attention_output": attention_output, "mask_list": mask_list})
-        self.last_edit_controllers = edits
         return results
+
+    # ---- several source clips in one pass (test_fatezero_dataset.py sweeps clip after clip) --------------------------------------
+    def _engine_is_sharded(self) -> bool:
+        engine = getattr(self.unet, "_engine", None)  # not built here: nothing may touch the GPU before the checks pass
+        return getattr(engine, "shard", None) is not None
+
+    def map_cache_admission(self, clips: int, frames: int, h: int, w: int, steps: int, save_self_attention: bool = True,
+                            free_bytes: Optional[int] = None) -> int:
+        """Bytes of the inversion map caches of `clips` clips of `frames` frames at latent size h x w over `steps` DDIM steps (the slab
+        shapes of controllers.map_cache_bytes).  Raises ValueError when they exceed `free_bytes` (default: the free HBM of the UNet's
+        device plus the blocks PyTorch holds unused)."""
+        per_step, once = attention_util.map_cache_bytes(dict(self.unet.config), dict(self.unet.model_config), h, w, save_self_attention)
+        need = clips * frames * (steps * per_step + once)
+        if free_bytes is None:
+            dev = self.unet.device
+            if dev.type != "cuda":
+                return need
+            free_bytes = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+        if need > free_bytes:
+            raise ValueError(f"the inversion map caches of {clips} clips x {frames} frames x {steps} steps need {need / 2 ** 30:.1f} GiB, "
+                             f"{free_bytes / 2 ** 30:.1f} GiB of HBM are free: invert the clips in smaller batches")
+        return need
+
+    @torch.no_grad()
+    def prepare_latents_ddim_inverted_batch(self, source_prompts: List[str], images=None, latents=None, generator=None,
+                                            store_attention: bool = True):
+        """DDIM-invert K source clips in ONE batched pass (p2p_ddim_spatial_temporal.py:68-129 once per clip, as test_fatezero_dataset.py
+        does): every UNet forward runs the K clips together, each with its own attention store.  `images`: K frame tensors [F, 3, H, W]
+        (VAE-encoded clip by clip with `generator`, one generator or a list of K) or `latents`: K clean latents [1, 4, F, h, w].  The
+        scheduler's current timesteps are used, as by prepare_latents_ddim_inverted.
+
+        Clip k's N+1 latents, and the state of its store (`attention_store_all_step`, `attention_store`, `latents_store`, `cur_step`), are
+        bit for bit those of prepare_latents_ddim_inverted(..., store_attention=store_attention) on that clip alone.  Returns the K lists
+        of N+1 latents ([0] clean, [-1] x_T) and sets `self.store_controllers` to the K stores."""
+        source_prompts = list(source_prompts)
+        K = len(source_prompts)
+        if (images is None) == (latents is None):
+            raise ValueError("prepare_latents_ddim_inverted_batch: pass either images or latents")
+        clips = list(images if images is not None else latents)
+        if K == 0 or len(clips) != K:
+            raise ValueError(f"prepare_latents_ddim_inverted_batch: {K} source prompts and {len(clips)} clips")
+        if K > attention_util._lib.MAX_ATTN_GROUPS:
+            raise ValueError(f"prepare_latents_ddim_inverted_batch: at most {attention_util._lib.MAX_ATTN_GROUPS} clips per batch, got {K}")
+        if images is not None:
+            if any(c.dim() != 4 for c in clips):
+                raise ValueError("prepare_latents_ddim_inverted_batch: images must be frame tensors [F, 3, H, W]")
+            geo = [(c.shape[0], c.shape[2] // self.vae_scale_factor, c.shape[3] // self.vae_scale_factor) for c in clips]
+        else:
+            if any(c.dim() != 5 or c.shape[0] != 1 for c in clips):
+                raise ValueError("prepare_latents_ddim_inverted_batch: latents must be clean latents [1, 4, F, h, w]")
+            geo = [(c.shape[2], c.shape[3], c.shape[4]) for c in clips]
+        if len(set(geo)) != 1:
+            raise ValueError(f"prepare_latents_ddim_inverted_batch: the clips differ in (frames, h, w): {geo}; batch clips of one geometry")
+        F, h, w = geo[0]
+        if K * F > self.MAX_BATCH_ROWS:
+            raise ValueError(f"prepare_latents_ddim_inverted_batch: {K} clips x {F} frames = {K * F} rows exceed {self.MAX_BATCH_ROWS}")
+        if self._engine_is_sharded():
+            raise NotImplementedError("prepare_latents_ddim_inverted_batch: frame-sharded batched inversions are not supported")
+        stores = [] if self.store_controller.disk_store else [attention_util.AttentionStore() for _ in range(K)]
+        if not stores or any(s.host_spill for s in stores):
+            raise NotImplementedError("prepare_latents_ddim_inverted_batch: disk_store / host_spill stores are inverted one clip at a time")
+        gens = list(generator) if isinstance(generator, list) else [generator] * K
+        if len(gens) != K:
+            raise ValueError(f"prepare_latents_ddim_inverted_batch: {len(gens)} generators for {K} clips")
+        N = len(self.scheduler.timesteps)
+        batch = attention_util.AttentionStoreBatch(stores, store_maps=store_attention)
+        for s in stores:
+            s.LOW_RESOURCE = True  # before the plan signature is read: a captured inversion was keyed with it set
+        # the previous batch's stores are let go before the admission counts the free HBM (a caller still holding them keeps their caches);
+        # a batch that will replay a captured inversion refills that plan's caches and allocates none
+        self.store_controllers = None
+        replays = self.graph_mode != "off" and any(
+            k[0] == "inv" and k[1] == (K, 4, F, h, w) and k[3] == tuple(int(t) for t in self.scheduler.timesteps) and k[5] == batch.graph_signature()
+            for k in self._plans)
+        if store_attention and not replays:
+            self.map_cache_admission(K, F, h, w, N)
+        self.prepare_before_train_loop()
+        if images is not None:
+            # clip by clip: the VAE's GroupNorm chunking depends on the batch
+            clean = []
+            for img, g in zip(clips, gens):
+                z = 0.18215 * self._vae_encode_sample(img, g)
+                clean.append(z.reshape(1, F, *z.shape[1:]).permute(0, 2, 1, 3, 4))
+        else:
+            clean = clips
+        dev = self.unet.device
+        per = [self._encode_prompt(p, dev, 1, True, None).to(dev) for p in source_prompts]
+        text = torch.cat([e[:1] for e in per] + [e[1:] for e in per])
+        attention_util.register_attention_control(self, batch)
+        try:
+            out = self.ddim_clean2noisy_loop(torch.cat(clean), text, batch)
+        finally:
+            attention_util.register_attention_control(self, self.empty_controller)
+            for s in stores:
+                s.LOW_RESOURCE = False
+        self.store_controllers = stores
+        return [[c] + [o[k:k + 1] for o in out[1:]] for k, c in enumerate(clean)]
+
+    @torch.no_grad()
+    def p2preplace_edit_clips(self, jobs: List[dict], num_inference_steps: int, guidance_scale: float, output_type: str = "pil",
+                              save_path: Optional[str] = None, negative_prompt=None, callback=None, callback_steps: int = 1):
+        """Edit several inverted clips in ONE batched pass (p2p_ddim_spatial_temporal.py:172-222 once per job).  Each job is
+        dict(store=<the clip's AttentionStore>, latents=<its x_T [1, 4, F, h, w]>, prompt=..., source_prompt=..., **p2p_config); any
+        number of jobs may edit the same clip.  Job j gets, bit for bit, what p2preplace_edit(prompt=..., **p2p_config) gives it against
+        its own store (latents, masks, running attention sums).  Returns one p2preplace_edit result dict per job (VAE decode per job);
+        `self.last_edit_controllers` holds the edit controllers.  callback(i, t, latents[J, ...])."""
+        jobs = [dict(j) for j in jobs]
+        J = len(jobs)
+        if J == 0:
+            raise ValueError("p2preplace_edit_clips: no jobs")
+        if J > attention_util._lib.MAX_ATTN_GROUPS:
+            raise ValueError(f"p2preplace_edit_clips: at most {attention_util._lib.MAX_ATTN_GROUPS} jobs per batch, got {J}")
+        for k, j in enumerate(jobs):
+            missing = [n for n in ("store", "latents", "prompt", "source_prompt") if j.get(n) is None]
+            if missing:
+                raise ValueError(f"p2preplace_edit_clips: job {k} lacks {missing}")
+            if j["latents"].dim() != 5 or j["latents"].shape[0] != 1:
+                raise ValueError(f"p2preplace_edit_clips: job {k}: latents must be the clip's x_T of shape [1, 4, F, h, w]")
+        shapes = [tuple(j["latents"].shape) for j in jobs]
+        if len(set(shapes)) != 1:
+            raise ValueError(f"p2preplace_edit_clips: the clips differ in shape {shapes}; batch clips of one (frames, h, w)")
+        F = shapes[0][2]
+        if 2 * J * F > self.MAX_BATCH_ROWS:
+            raise ValueError(f"p2preplace_edit_clips: 2 x {J} jobs x {F} frames = {2 * J * F} CFG rows exceed {self.MAX_BATCH_ROWS}")
+        for k, j in enumerate(jobs):
+            if int(j.get("num_inference_steps", num_inference_steps)) != int(num_inference_steps):
+                raise ValueError(f"p2preplace_edit_clips: job {k} asks for num_inference_steps={j['num_inference_steps']}")
+            if float(j.get("guidance_scale", guidance_scale)) != float(guidance_scale):
+                raise ValueError(f"p2preplace_edit_clips: job {k} asks for guidance_scale={j['guidance_scale']}")
+            if float(j.get("eta", 0.0)) != 0.0:
+                raise NotImplementedError("FateZero's DDIM path is deterministic (eta = 0)")
+            st = j["store"]
+            if getattr(st, "disk_store", False) or getattr(st, "host_spill", False):
+                raise NotImplementedError("p2preplace_edit_clips: disk_store / host_spill inversion stores are edited one clip at a time")
+            if len(st.attention_store_all_step) != int(num_inference_steps):
+                raise ValueError(f"p2preplace_edit_clips: job {k}'s store holds {len(st.attention_store_all_step)} inversion steps, the edit "
+                                 f"runs {num_inference_steps}; batch clips inverted with one step count")
+        stores = list({id(j["store"]): j["store"] for j in jobs}.values())
+        plans = [s._graph_plan_id for s in stores if getattr(s, "_graph_plan_id", None) is not None]
+        if len(set(plans)) != len(plans):
+            raise ValueError("p2preplace_edit_clips: two stores hold the maps of the same captured inversion slot; only the clip inverted last "
+                             "by that plan still has its maps")
+        if self._engine_is_sharded():
+            raise NotImplementedError("p2preplace_edit_clips: frame-sharded batched edits are not supported")
+        drop = ("store", "latents", "prompt", "source_prompt", "num_inference_steps", "guidance_scale", "eta", "save_path", "output_type",
+                "negative_prompt", "callback", "callback_steps")
+        edits = [self._make_edit_controller(prompt=j["prompt"], source_prompt=j["source_prompt"], num_inference_steps=num_inference_steps,
+                                            save_path=save_path, store=j["store"], **{k: v for k, v in j.items() if k not in drop})
+                 for j in jobs]
+        ctrl = attention_util.AttentionControlEditClips(edits)
+        prompts = [j["prompt"] for j in jobs]
+        attention_util.register_attention_control(self, ctrl)
+        try:
+            out = self.sd_ddim_pipeline(prompt=prompts, num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
+                                        negative_prompt=negative_prompt, latents=torch.cat([j["latents"] for j in jobs]), output_type="latent",
+                                        callback=callback, callback_steps=callback_steps, controller=ctrl)
+        finally:
+            attention_util.register_attention_control(self, self.empty_controller)
+        self.last_edit_controllers = edits
+        return self._batch_results(prompts, edits, out.images, output_type)
 
     @torch.no_grad()
     def __call__(self, **kwargs):
@@ -522,6 +688,7 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         if not do_cfg:
             raise NotImplementedError("guidance_scale <= 1 (no CFG batch) is not an editing configuration of the reference YAMLs")
         is_batch = isinstance(controller, attention_util.AttentionControlEditBatch)
+        is_clips = isinstance(controller, attention_util.AttentionControlEditClips)
         if is_batch:
             # K prompts of one clip: [uncond_1..K ; cond_1..K], each prompt encoded on its own so that its embedding is bitwise the one of
             # its single-prompt pass
@@ -530,7 +697,7 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
             negs = negative_prompt if isinstance(negative_prompt, list) else [negative_prompt] * len(prompt)
             per = [self._encode_prompt(pr, device, 1, do_cfg, ng).to(self.unet.device) for pr, ng in zip(prompt, negs)]
             text_embeddings = torch.cat([e[:1] for e in per] + [e[1:] for e in per])
-            if latents.shape[0] == 1:
+            if latents.shape[0] == 1 and not is_clips:
                 latents = latents.expand(len(prompt), *latents.shape[1:])
         else:
             text_embeddings = self._encode_prompt(prompt, device, num_images_per_prompt, do_cfg, negative_prompt).to(self.unet.device)
@@ -559,7 +726,10 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
             eps2 = self.unet(x2, t, encoder_hidden_states=text).sample
             blend = ctrl.latent_blend_args(x.shape[-2], x.shape[-1]) if is_edit else None
             a_t, a_prev = self._alpha(t), self._alpha(t - step)
-            if is_batch:
+            if is_clips:
+                ops.cfg_ddim_step_multi(x, eps2.contiguous(), guidance_scale, a_t, a_prev,
+                                        blends=[None if b is None else dict(b, x_inv=b["x_inv"].contiguous()) for b in blend])
+            elif is_batch:
                 live = [b for b in blend if b is not None]
                 x_inv = live[0]["x_inv"].contiguous() if live else None
                 if any(b["x_inv"].data_ptr() != live[0]["x_inv"].data_ptr() for b in live[1:]):

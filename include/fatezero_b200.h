@@ -117,7 +117,8 @@ int fz_attention_f16(const fz_attn_args_t* args, fz_stream_t stream);
  * [uncond_1..K ; cond_1..K].  Rows bf >= args->edit_bf_start belong to group g = (bf - edit_bf_start) / F and read cache frame
  * fc = (bf - edit_bf_start) % F of the SAME `base` slab [F, heads, S_q, cache_ld] (the inversion map of the step); BF - edit_bf_start
  * must equal n_groups * F.  The per-row hook fields of `args` (row_mode, xedit, mask, acc) are ignored: each group brings its own.
- * Modes NONE / REPLACE / BLEND / CROSSEDIT may be mixed in one launch; STORE is refused.  BF <= 128 (fz_attention_f16: BF <= 64).
+ * Modes NONE / REPLACE / BLEND / CROSSEDIT / STORE may be mixed in one launch (STORE groups all write args->store: use
+ * fz_attention_grouped_slabs_f16 below to give each its own slab).  BF <= 128 (fz_attention_f16: BF <= 64).
  * Every row computes exactly what fz_attention_f16 computes for it with its group's hook, so each group's rows and `acc` are bitwise
  * equal to a launch over that group alone. */
 #define FZ_ATTN_MAX_GROUPS 8
@@ -132,6 +133,19 @@ typedef struct fz_attn_groups {
   fz_attn_group_t g[FZ_ATTN_MAX_GROUPS];
 } fz_attn_groups_t;
 int fz_attention_grouped_f16(const fz_attn_args_t* args, const fz_attn_groups_t* groups, fz_stream_t stream);
+
+/* The grouped launch with a cache slab per group, so that groups of different clips share one launch: the batched inversion of
+ * several clips (p2p_ddim_spatial_temporal.py:68-129 once per clip in test_fatezero_dataset.py; one STORE group of F rows per clip,
+ * edit_bf_start = 0) and the batched edit of several clips (:172-222; each group reads the inversion map of its own clip).  Group g
+ * writes (STORE) cache frame fc = (bf - edit_bf_start) % F of store[g] and adds to its own running sum groups->g[g].acc; REPLACE /
+ * BLEND / CROSSEDIT read base[g].  A NULL entry means the slab of `args` (store / base), so `slabs` == NULL or all-NULL is exactly
+ * fz_attention_grouped_f16.  Every slab has the geometry [F, heads, S_q, args->cache_ld].  STORE may be mixed with the other modes. */
+typedef struct fz_attn_slabs {
+  void* store[FZ_ATTN_MAX_GROUPS];       /* STORE: cache slab written by group g, or NULL                                    */
+  const void* base[FZ_ATTN_MAX_GROUPS];  /* REPLACE / BLEND / CROSSEDIT: cached source map read by group g, or NULL             */
+} fz_attn_slabs_t;
+int fz_attention_grouped_slabs_f16(const fz_attn_args_t* args, const fz_attn_groups_t* groups, const fz_attn_slabs_t* slabs,
+                                   fz_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * HBM-bound kernels of the step
@@ -181,6 +195,12 @@ int fz_cfg_ddim_step(float* x, const float* eps2, long long n, float guidance, f
 int fz_cfg_ddim_step_batched(float* x, const float* eps2, int K, long long n_item, float guidance, float alpha_t, float alpha_prev,
                              const float* x_inv, const float* const* mask_a, const float* const* mask_b, const int* apply_blend,
                              long long fhw, fz_stream_t stream);
+/* The same step for K <= 8 items of possibly different clips (the edit jobs of p2preplace_edit_clips: :400-407 once per clip): x_inv is a
+ * HOST array [K] of device pointers, one inverted latent [n_item] per item (two items may share one; NULL where an item does not blend).
+ * Item k gets exactly the arithmetic of fz_cfg_ddim_step on its slice with x_inv[k]. */
+int fz_cfg_ddim_step_multi(float* x, const float* eps2, int K, long long n_item, float guidance, float alpha_t, float alpha_prev,
+                           const float* const* x_inv, const float* const* mask_a, const float* const* mask_b, const int* apply_blend,
+                           long long fhw, fz_stream_t stream);
 /* blend mask from cached cross maps (spatial_blend.py:24-39,78-111); maps: HOST array of device pointers, word_w: HOST [ntok] */
 int fz_blend_mask(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int r, int ldm, int ntok, const float* word_w,
                   float th, int h, int w, float* out, fz_stream_t stream);
