@@ -13,10 +13,19 @@ Tap-GEMM outputs (GEMM, conv3x3, tconv3: fp32 accumulation, one rounding to fp16
 
 Attention outputs (P rounded to fp16 before PV, fp32 accumulation) pass when
 
-    |got - ref64| <= 2^-11 * sum_t p_t |v_t| + 2^-25 * sum_t |v_t| + ulp16(O)
+    |got - ref64| <= 2^-11 * sum_t |p_t| |v_t| + 2^-25 * sum_t |v_t| + ulp16(O)
 
   the middle term covers P entries in the fp16 subnormal range, whose rounding error is absolute (<= 2^-25), not relative; the kernels
   divide by a row sum >= 1, so it is not amplified.
+
+The cross-attention edit (CROSSEDIT of fz_attn.cu: Refine / Replace, Reweight, alpha-lerp in fp32, one rounding to fp16) is built from the
+stored fp16 P, the fp16 cached source rows and the fp32 tables, and passes when
+
+    |got - ref64| <= ulp16(ref64) + c * 2^-24 * sum|terms|
+
+  the terms being the edit evaluated on absolute values, with a factor keys_per_slot on the Replace sum (its running fp32 sum).
+The fp16 running sums of the cross maps are checked bitwise: acc_new = acc_old + P_store in fp16 (one fp32 add, one rounding), the
+columns past keys_per_slot unchanged.
 
 GroupNorm / LayerNorm outputs (test_gpu_elem_edges.py): y = gamma (x - mu) rstd + beta, rstd = 1 / sqrt(var + eps), mu and var the fp64
 statistics of the fp16 inputs, pass when
@@ -144,9 +153,10 @@ def softmax64(s: torch.Tensor) -> torch.Tensor:
 
 
 def attn_bound(p: torch.Tensor, v: torch.Tensor, o: torch.Tensor) -> torch.Tensor:
-    """p [..., S, T] fp64 probabilities, v [..., T, d] fp64, o = p @ v: the attention bound of the module docstring."""
+    """p [..., S, T] fp64 probabilities, v [..., T, d] fp64, o = p @ v: the attention bound of the module docstring.  |p|: an edited row
+    (CROSSEDIT with a negative equalizer) has negative entries, and each entry's rounding error scales with its magnitude."""
     va = v.abs()
-    return U16 * (p @ va) + 2.0 ** -25 * va.sum(-2, keepdim=True) + ulp16(o)
+    return U16 * (p.abs() @ va) + 2.0 ** -25 * va.sum(-2, keepdim=True) + ulp16(o)
 
 
 def check_attn(got, p, v, report=None, key="") -> dict:
@@ -159,6 +169,90 @@ def check_probs(got, p, report=None, key="", k_ulp: float = 1.0) -> dict:
     """Stored probabilities: within k_ulp fp16 ulps of fp16(softmax64)."""
     r = p.double().half().double()
     return check_bound(got, r, k_ulp * ulp16(r), report, key)
+
+
+# ---------------------------------------------------------------------------------------------------------- cross-attention edit
+# Layout of the CROSSEDIT table (include/fatezero_b200.h): [0] mode (0 refine, 1 replace), then alpha[80], eq[80], a[80], mapper[80] and
+# M[80][80] (M[w][n]: source word w into target word n).
+XEDIT_FLOATS = 8 + 4 * 80 + 80 * 80
+X_ALPHA, X_EQ, X_A, X_MAP, X_M = 8, 88, 168, 248, 328
+
+# c of the edit bound: the running-error bound of the few fp32 operations after the gather / sum (eq, the lerp's product and sum).
+# Measured on an H100 80GB HBM3 (700 W power limit) over every case of test_gpu_attn_edges.py that edits (each records its own
+# c_needed): the largest c any case needed was 0 (every edited P within 0.5 ulp of the fp64 edit, worst err / bound 0.50).
+C_EDIT = 4.0
+
+
+def cross_edit_table(kind: str, kps: int) -> torch.Tensor:
+    """A CROSSEDIT table (fp32, CPU) for keys_per_slot = kps whose entries tell the edit's operations apart:
+    alpha cycles through 0, 1 and fractional values, eq through 1, 0, -1, 2.5, 10 and 0.5 (so eq != 1 meets every kind of alpha);
+    kind "refine": fractional a, a mapper with entries -1 where a != 0;  "reweight": identity mapper, a = 1 (pure Reweight);
+    "replace": M with one-to-many and many-to-one columns and non-zero rows past 64 when kps > 64 (Reweight on Replace)."""
+    n = torch.arange(80)
+    t = torch.zeros(XEDIT_FLOATS)
+    t[0] = 1.0 if kind == "replace" else 0.0
+    t[X_ALPHA:X_ALPHA + 80] = torch.tensor([0.0, 1.0, 0.375, 1.0, 0.3])[n % 5]
+    t[X_EQ:X_EQ + 80] = torch.tensor([1.0, 0.0, -1.0, 2.5, 10.0, 1.0, 0.5])[n % 7]
+    if kind == "reweight":
+        t[X_A:X_A + 80] = 1.0
+        t[X_MAP:X_MAP + 80] = n.float()
+    elif kind == "refine":
+        a = torch.tensor([0.0, 1.0, 0.25, 0.7])[n % 4]
+        mp = (7 * n + 3) % kps
+        for i in (2, 11):  # a = 0.25, 0.7: the gather of word -1 (python: the last word) is visible
+            mp[i] = -1
+        t[X_A:X_A + 80] = a
+        t[X_MAP:X_MAP + 80] = mp.float()
+    else:
+        M = torch.zeros(80, 80)
+        k = torch.arange(kps)
+        M[(5 * k + 1) % kps, k] = 0.625
+        M[(11 * k + 7) % kps, k] += 0.375
+        M[kps - 3:kps, 3] = 0.5          # many-to-one: the last three words into word 3
+        M[kps - 5, :min(kps, 10)] += 0.3  # one-to-many: one late word into words 0..9
+        t[X_M:] = M.reshape(-1)
+    return t
+
+
+def cross_edit_ref(cur, base, table, kps: int):
+    """fz_attn.cu CROSSEDIT in fp64: cur [..., S, >= kps] the fp16 probabilities the kernel edits (stored P), base [..., S, >= kps] the fp16
+    cached source rows, table the fp32 CROSSEDIT table ->  (ref, sum|terms|) [..., S, kps] fp64, before the final fp16 rounding:
+        Refine   R = b[map[n] mod kps] a[n] + cur (1 - a[n])          Replace   R = sum_{w < kps} b[w] M[w][n]
+        then     R = R eq[n],  x = R al[n] + (1 - al[n]) cur."""
+    t = table.double().to(cur.device)
+    c, b = cur[..., :kps].double(), base[..., :kps].double()
+    al, eq = t[X_ALPHA:X_ALPHA + kps], t[X_EQ:X_EQ + kps]
+    if t[0].item() == 1.0:
+        M = t[X_M:].view(80, 80)[:kps, :kps]
+        R, T = b @ M, kps * (b.abs() @ M.abs())
+    else:
+        a, mp = t[X_A:X_A + kps], t[X_MAP:X_MAP + kps].long() % kps
+        R = b[..., mp] * a + c * (1 - a)
+        T = b[..., mp].abs() * a.abs() + c.abs() * (1 - a).abs()
+    R, T = R * eq, T * eq.abs()
+    return R * al + (1 - al) * c, T * al.abs() + (1 - al).abs() * c.abs()
+
+
+def check_edit(got, ref, terms, report=None, key="", c: float = C_EDIT) -> dict:
+    """Edited probabilities against cross_edit_ref (bound: module docstring).  Also records c_needed: the smallest c this case passes with."""
+    ref, terms = ref.double(), terms.double()
+    u = ulp16(ref)
+    acc = U32 * terms
+    err = (got.double() - ref).abs()
+    c_needed = ((err - u).clamp(min=0) / acc.clamp(min=1e-300)).max().item()
+    return check_bound(got, ref, u + c * acc, report, key, extra=dict(c_needed=c_needed, c=c))
+
+
+def check_running_sum(new, old, p16, kps: int, report=None, key="") -> dict:
+    """fp16 running sum [..., S, acc_ld] after one add: columns < kps bitwise equal to old + p16 (fp16 tensors: one fp32 add, one rounding,
+    which is the kernel's fp16(fp32(acc) + fp32(fp16 p)) and the reference's fp16 +=), columns >= kps bitwise unchanged."""
+    want = old[..., :kps] + p16[..., :kps]
+    bad_sum = int((new[..., :kps] != want).sum().item())
+    bad_pad = int((new[..., kps:] != old[..., kps:]).sum().item())
+    stats = dict(n=new.numel(), sum_mismatches=bad_sum, pad_changed=bad_pad)
+    _record(report, key, stats)
+    assert bad_sum == 0 and bad_pad == 0, f"{key}: running sum differs from old + P in {bad_sum} elements, {bad_pad} pad columns changed"
+    return stats
 
 
 # ---------------------------------------------------------------------------------------------------------------- normalisation

@@ -8,8 +8,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from _ref64 import (blend_mask_ratio, cfg_ddim_ref, check_attn, check_heatmaps, check_mask, check_probs, check_step, check_tap, ddim_invert_ref,
-                    gemm_ref, gn_check, heatmap_values, ln_check, nearest_index, softmax64, ulp16)
+from _ref64 import (X_A, X_ALPHA, X_EQ, X_M, X_MAP, blend_mask_ratio, cfg_ddim_ref, check_attn, check_edit, check_heatmaps, check_mask,
+                    check_probs, check_running_sum, check_step, check_tap, cross_edit_ref, cross_edit_table, ddim_invert_ref, gemm_ref, gn_check,
+                    heatmap_values, ln_check, nearest_index, softmax64, ulp16)
 
 
 def rnd(*shape, seed=0, scale=1.0):
@@ -82,6 +83,9 @@ def test_attn_accepts_fp16_p_and_exact():
     check_attn((p @ v64).half(), p, v64)
     check_attn((p.half().double() @ v64).half(), p, v64)
     check_probs(p.half(), p)
+    # an edited row (negative equalizer): signed entries, each rounded to fp16
+    ps = p * 10 * torch.where(torch.arange(p.shape[-1]) % 3 == 0, -1.0, 1.0).double()
+    check_attn((ps.half().double() @ v64).half(), ps, v64)
 
 
 def test_attn_rejects_missing_key_block():
@@ -238,6 +242,103 @@ def test_heatmaps_reject_white_zero_column():
     bad[:, 9] = 255  # fminf(255, 0/0) on a column whose maximum is 0
     with pytest.raises(AssertionError, match="differ"):
         check_heatmaps(bad, v)
+
+
+# ------------------------------------------------------------------------------------------------------------ cross-attention edit
+def edit_case(kind, kps=77, S=48):
+    cur = softmax64(rnd(2, S, kps, seed=90) * 2).half()
+    base = softmax64(rnd(2, S, kps, seed=91) * 2).half()
+    return cur, base, cross_edit_table(kind, kps)
+
+
+def with_table(t, **rows):
+    """A copy of table t with the named ranges replaced: alpha / eq / a / mapper [80], M [80, 80]."""
+    t = t.clone()
+    for name, v in rows.items():
+        off = dict(alpha=X_ALPHA, eq=X_EQ, a=X_A, mapper=X_MAP, M=X_M)[name]
+        v = v.reshape(-1)
+        t[off:off + v.numel()] = v
+    return t
+
+
+@pytest.mark.parametrize("kind", ["refine", "replace", "reweight"])
+@pytest.mark.parametrize("kps", [77, 16, 80])
+def test_edit_accepts_correct_rounding(kind, kps):
+    cur, base, t = edit_case(kind, kps)
+    ref, terms = cross_edit_ref(cur, base, t, kps)
+    check_edit(ref.half(), ref, terms)
+    # at alpha = 0 the edit is the current probability, whatever eq
+    al = t[X_ALPHA:X_ALPHA + kps]
+    assert torch.equal(ref[..., al == 0], cur[..., :kps][..., al == 0].double())
+
+
+def eq_after_lerp(cur, base, t, kps):
+    x, _ = cross_edit_ref(cur, base, with_table(t, eq=torch.ones(80)), kps)
+    return x * t[X_EQ:X_EQ + kps].double()
+
+
+def m_transposed(cur, base, t, kps):
+    return cross_edit_ref(cur, base, with_table(t, M=t[X_M:].view(80, 80).t()), kps)[0]
+
+
+def replace_first_atom(cur, base, t, kps):
+    M = t[X_M:].view(80, 80).clone()
+    M[64:] = 0
+    return cross_edit_ref(cur, base, with_table(t, M=M), kps)[0]
+
+
+def mapper_minus1_as_0(cur, base, t, kps):
+    mp = t[X_MAP:X_MAP + 80]
+    return cross_edit_ref(cur, base, with_table(t, mapper=torch.where(mp < 0, torch.zeros_like(mp), mp)), kps)[0]
+
+
+def alpha_swapped(cur, base, t, kps):
+    return cross_edit_ref(cur, base, with_table(t, alpha=1 - t[X_ALPHA:X_ALPHA + 80]), kps)[0]
+
+
+def refine_lerp_reversed(cur, base, t, kps):
+    return cross_edit_ref(cur, base, with_table(t, a=1 - t[X_A:X_A + 80]), kps)[0]
+
+
+@pytest.mark.parametrize("kind,bug", [("refine", eq_after_lerp), ("replace", eq_after_lerp), ("reweight", eq_after_lerp),
+                                      ("replace", m_transposed), ("replace", replace_first_atom), ("refine", mapper_minus1_as_0),
+                                      ("refine", alpha_swapped), ("replace", alpha_swapped), ("refine", refine_lerp_reversed)],
+                         ids=lambda v: v if isinstance(v, str) else v.__name__)
+def test_edit_rejects(kind, bug):
+    cur, base, t = edit_case(kind)
+    ref, terms = cross_edit_ref(cur, base, t, 77)
+    with pytest.raises(AssertionError, match="out of bound"):
+        check_edit(bug(cur, base, t, 77).half(), ref, terms)
+
+
+def test_edit_rejects_3ulp_move():
+    cur, base, t = edit_case("replace")
+    ref, terms = cross_edit_ref(cur, base, t, 77)
+    got = ref.half().flatten().clone()
+    i = int(terms.flatten().argmax())  # where the bound is widest
+    got[i] = (got[i].double() + 3 * ulp16(got[i].double())).half()
+    with pytest.raises(AssertionError, match="out of bound"):
+        check_edit(got.view_as(ref), ref, terms)
+
+
+def test_running_sum_rejects_edited_p_and_unrounded_add():
+    cur, base, t = edit_case("refine")
+    p64 = softmax64(rnd(2, 48, 77, seed=90) * 2)  # cur before its rounding to fp16
+    old = (4 + 4 * torch.rand(2, 48, 96, generator=torch.Generator().manual_seed(92))).half()
+    pad = torch.zeros(2, 48, 96, dtype=torch.float16)
+    pad[..., :77] = cur
+    check_running_sum(old + pad, old, cur, 77)
+    edited = cross_edit_ref(cur, base, t, 77)[0].half()
+    with pytest.raises(AssertionError, match="differs"):
+        check_running_sum(old + torch.cat([edited, pad[..., 77:]], -1), old, cur, 77)
+    unrounded = old.clone()
+    unrounded[..., :77] = (old[..., :77].double() + p64).half()  # the fp32 probability added before its rounding to fp16
+    with pytest.raises(AssertionError, match="differs"):
+        check_running_sum(unrounded, old, cur, 77)
+    touched = old + pad
+    touched[..., 80] += 1  # a pad column written
+    with pytest.raises(AssertionError, match="pad columns changed"):
+        check_running_sum(touched, old, cur, 77)
 
 
 def test_step_rejects_guidance_on_wrong_half():
