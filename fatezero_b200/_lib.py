@@ -85,6 +85,8 @@ SIGNATURES = {
     "fz_groupnorm_stats_f16": [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
     "fz_groupnorm_apply_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p,
                                c_void_p],
+    "fz_groupnorm_apply_sums64_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int,
+                                      c_void_p, c_void_p],
     "fz_layernorm_f16": [c_void_p, c_void_p, c_ll, c_int, c_void_p, c_void_p, c_float, c_void_p],
     "fz_upsample2x_nhwc_f16": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "fz_concat_channels_f16": [c_void_p, c_int, c_void_p, c_int, c_void_p, c_ll, c_void_p],
@@ -109,7 +111,7 @@ SIGNATURES = {
     "fz_p2p_unimport": [c_void_p],
     "fz_p2p_push": [C.POINTER(P2PSeg), c_int, C.POINTER(c_void_p), c_void_p, c_int, c_void_p, C.c_uint, c_void_p],
     "fz_p2p_wait": [c_void_p, C.c_uint, c_void_p],
-    "fz_gn_combine": [c_void_p, C.POINTER(c_void_p), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "fz_gn_combine": [c_void_p, C.POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "fz_softmax_rows_f16": [c_void_p, c_ll, c_int, c_ll, c_float, c_void_p],
     "fz_embed_tokens_f16": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     "fz_quick_gelu_f16": [c_void_p, c_ll, c_void_p],

@@ -141,8 +141,9 @@ __global__ void __launch_bounds__(kGnThreads) gn_stats_kernel(const __half* __re
 template <int SLOTS>
 __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(const __half* __restrict__ x, __half* __restrict__ y, int HW, int C, int G,
                                                              int frames_per_stat, int count_frames, int TX, int px_per_cta,
-                                                             const float2* __restrict__ image_sums, const float* __restrict__ gamma,
-                                                             const float* __restrict__ beta, float eps, int silu) {
+                                                             const float2* __restrict__ image_sums, const double2* __restrict__ image_sums64,
+                                                             const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                                                             int silu) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float s_mean[64], s_rstd[64];
@@ -152,9 +153,15 @@ __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(const __half* __re
     const int first = (nb / frames_per_stat) * frames_per_stat;
     double sa = 0.0, sb = 0.0;
     for (int i = 0; i < frames_per_stat; ++i) {
-      const float2 v = image_sums[(first + i) * G + threadIdx.x];
-      sa += v.x;
-      sb += v.y;
+      if (image_sums64) {  // fz_groupnorm_apply_sums64_f16: fp64 sums (the set totals of the frame-sharded exchange)
+        const double2 v = image_sums64[(first + i) * G + threadIdx.x];
+        sa += v.x;
+        sb += v.y;
+      } else {
+        const float2 v = image_sums[(first + i) * G + threadIdx.x];
+        sa += v.x;
+        sb += v.y;
+      }
     }
     const double cnt = static_cast<double>(cpg) * HW * count_frames;  // count_frames > frames_per_stat: frames held by other GPUs
     const double mean = sa / cnt;
@@ -778,11 +785,11 @@ static inline int grid_for(long long total, int threads) {
 
 using namespace fz;
 
-// which = 1: statistics only, 2: apply only (image_sums supplied by the caller), 3: both
+// which = 1: statistics only, 2: apply only (image_sums supplied by the caller: float2, or double2 when sums_f64), 3: both
 // geometry_images: the number of images the chunking is planned for (NB, or the images of one item of a batched edit)
 static int groupnorm_impl(int which, const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, int count_frames,
                           const float* gamma, const float* beta, float eps, int silu, void* workspace_f64, const void* sums_in,
-                          cudaStream_t stream, int geometry_images) {
+                          cudaStream_t stream, int geometry_images, bool sums_f64 = false) {
   if (int rc = check_single_device()) return rc;
   FZ_CHECK_ARG(C % 8 == 0 && C % groups == 0 && groups <= 64, "fz_groupnorm: C=%d groups=%d unsupported", C, groups);
   FZ_CHECK_ARG(frames_per_stat >= 1 && NB % frames_per_stat == 0, "fz_groupnorm: NB %% frames_per_stat != 0");
@@ -803,7 +810,8 @@ static int groupnorm_impl(int which, const void* x, void* y, int NB, int HW, int
   float2* partial = static_cast<float2*>(workspace_f64);
   float2* image_sums = workspace_f64 ? reinterpret_cast<float2*>(static_cast<uint8_t*>(workspace_f64) + kGnStatsOffset) : nullptr;
   unsigned* counters = workspace_f64 ? reinterpret_cast<unsigned*>(static_cast<uint8_t*>(workspace_f64) + kGnCounterOffset) : nullptr;
-  const float2* sums = sums_in ? static_cast<const float2*>(sums_in) : image_sums;
+  const float2* sums = sums_in && !sums_f64 ? static_cast<const float2*>(sums_in) : image_sums;
+  const double2* sums64 = sums_f64 ? static_cast<const double2*>(sums_in) : nullptr;
   const __half* xh = static_cast<const __half*>(x);
   __half* yh = static_cast<__half*>(y);
 #define FZ_GN_LAUNCH(SL)                                                                                                             \
@@ -813,7 +821,7 @@ static int groupnorm_impl(int which, const void* x, void* y, int NB, int HW, int
                          image_sums, counters));                                                                                     \
     if (which & 2)                                                                                                                    \
       FZ_CUDA(launch_pdl(gn_apply_kernel<SL>, dim3(chunks_apply, NB), dim3(kGnThreads), 0, stream, xh, yh, HW, C, groups,               \
-                         frames_per_stat, count_frames, TX, ppc_apply, sums, gamma, beta, eps, silu));                               \
+                         frames_per_stat, count_frames, TX, ppc_apply, sums, sums64, gamma, beta, eps, silu));                      \
   } while (0)
   if (slots == 1) FZ_GN_LAUNCH(1);
   else if (slots == 2) FZ_GN_LAUNCH(2);
@@ -842,7 +850,8 @@ extern "C" int fz_groupnorm_batched_nhwc_f16(const void* x, void* y, int NB, int
 }
 
 // Frame-sharded GroupNorm (SURVEY.md 8(e)): statistics and apply as separate calls so that the (sum, sumsq) of the frames held by other
-// GPUs can be all-reduced in between.  fz_groupnorm_stats_f16 leaves float2 sums[NB][groups] at workspace + 768 KiB.
+// GPUs can be all-reduced in between.  fz_groupnorm_stats_f16 leaves float2 sums[NB][groups] at workspace + 768 KiB; the apply reads
+// float2 sums (fz_groupnorm_apply_f16) or double2 sums (fz_groupnorm_apply_sums64_f16: fz_gn_combine's fp64 set totals).
 extern "C" int fz_groupnorm_stats_f16(const void* x, int NB, int HW, int C, int groups, void* workspace_f64, cudaStream_t stream) {
   FZ_CHECK_ARG(x && workspace_f64, "fz_groupnorm_stats: null pointer");
   return groupnorm_impl(1, x, nullptr, NB, HW, C, groups, 1, 1, nullptr, nullptr, 0.f, 0, workspace_f64, nullptr, stream, NB);
@@ -853,6 +862,14 @@ extern "C" int fz_groupnorm_apply_f16(const void* x, void* y, int NB, int HW, in
                                       cudaStream_t stream) {
   FZ_CHECK_ARG(x && y && gamma && beta && image_sums && count_frames >= frames_per_stat, "fz_groupnorm_apply: bad arguments");
   return groupnorm_impl(2, x, y, NB, HW, C, groups, frames_per_stat, count_frames, gamma, beta, eps, silu, nullptr, image_sums, stream, NB);
+}
+
+extern "C" int fz_groupnorm_apply_sums64_f16(const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, int count_frames,
+                                             const float* gamma, const float* beta, float eps, int silu, const void* image_sums,
+                                             cudaStream_t stream) {
+  FZ_CHECK_ARG(x && y && gamma && beta && image_sums && count_frames >= frames_per_stat, "fz_groupnorm_apply: bad arguments");
+  return groupnorm_impl(2, x, y, NB, HW, C, groups, frames_per_stat, count_frames, gamma, beta, eps, silu, nullptr, image_sums, stream, NB,
+                        true);
 }
 
 extern "C" int fz_layernorm_f16(const void* x, void* y, long long M, int C, const float* gamma, const float* beta, float eps,

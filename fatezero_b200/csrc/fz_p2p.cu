@@ -105,14 +105,17 @@ __global__ void p2p_wait_kernel(unsigned* flags, unsigned mask) {
 // word carries its own validity and NO system fence or separate flag is needed (the fence pair + flag round trip of the generic exchange
 // cost 10-20 us per GroupNorm at 8 GPUs; this is one NVLink store latency).  The epoch is a per-site counter in local device memory that
 // every rank advances once per use (all ranks execute the same launch sequence), so the protocol is replay-safe inside CUDA graphs.
-// The receiver polls its own inbox, adds the peers' statistics to the local ones and leaves the total of every statistics set in the slot
-// of its first local image (the layout fz_groupnorm_apply_f16 consumes; the other slots of the set are zeroed).
+// The receiver polls its own inbox, adds the peers' statistics to the local ones and leaves the fp64 total of every statistics set in the
+// slot of its first local image of `totals` (the layout fz_groupnorm_apply_sums64_f16 consumes; the other slots of the set are zeroed).  The
+// totals stay in fp64, as the single-GPU apply keeps its fp64 sum of the per-image fp32 sums: a total rounded to fp32 moves the mean of a
+// constant group by up to 2^-24 |mean|, which rstd = eps^-1/2 turns into ~100 fp16 ulps of a small beta.
 // inbox: [world][NB * G][2] uint2 in this rank's arena (slot `me` unused); peer_inbox[r]: rank r's inbox slot for THIS rank.
 struct GnXchgParams {
   uint2* peer_inbox[32];
   const uint2* inbox;    // local
   unsigned* epoch;       // local per-site use counter
-  float2* sums;          // [NB * G] in / out
+  const float2* sums;    // [NB * G] this rank's per-image (sum, sumsq)
+  double2* totals;       // [NB * G] out: set totals in the first image of each set, 0 elsewhere
   int NB, F_loc, G, world, me;
 };
 __device__ __forceinline__ uint2 ld_relaxed_sys_v2(const uint2* p) {
@@ -171,8 +174,8 @@ __global__ void __launch_bounds__(1024) gn_combine_kernel(const __grid_constant_
       ta += gx_smem[2 * ((b * F_loc + f) * G + g)];
       tb += gx_smem[2 * ((b * F_loc + f) * G + g) + 1];
     }
-    p.sums[(b * F_loc) * G + g] = make_float2(static_cast<float>(ta), static_cast<float>(tb));
-    for (int f = 1; f < F_loc; ++f) p.sums[(b * F_loc + f) * G + g] = make_float2(0.f, 0.f);
+    p.totals[(b * F_loc) * G + g] = make_double2(ta, tb);
+    for (int f = 1; f < F_loc; ++f) p.totals[(b * F_loc + f) * G + g] = make_double2(0.0, 0.0);
   }
 }
 
@@ -253,9 +256,9 @@ extern "C" int fz_p2p_wait(void* flags, unsigned mask, cudaStream_t stream) {
   return FZ_OK;
 }
 
-extern "C" int fz_gn_combine(void* epoch, void* const* peer_inbox, const void* inbox, void* sums, int NB, int F_loc, int G, int world, int me,
-                             cudaStream_t stream) {
-  FZ_CHECK_ARG(epoch && peer_inbox && inbox && sums && F_loc >= 1 && NB % F_loc == 0 && world >= 1 && world <= 32 && me >= 0 && me < world,
+extern "C" int fz_gn_combine(void* epoch, void* const* peer_inbox, const void* inbox, const void* sums, void* totals, int NB, int F_loc, int G,
+                             int world, int me, cudaStream_t stream) {
+  FZ_CHECK_ARG(epoch && peer_inbox && inbox && sums && totals && F_loc >= 1 && NB % F_loc == 0 && world >= 1 && world <= 32 && me >= 0 && me < world,
                "fz_gn_combine: bad args");
   const int n = NB * G;
   FZ_CHECK_ARG(n <= 1024, "fz_gn_combine: %d images x groups > 1024", n);
@@ -266,7 +269,8 @@ extern "C" int fz_gn_combine(void* epoch, void* const* peer_inbox, const void* i
     FZ_CHECK_ARG(peer_inbox[r], "fz_gn_combine: null peer pointer");
     p.peer_inbox[r] = static_cast<uint2*>(peer_inbox[r]);
   }
-  p.inbox = static_cast<const uint2*>(inbox); p.epoch = static_cast<unsigned*>(epoch); p.sums = static_cast<float2*>(sums);
+  p.inbox = static_cast<const uint2*>(inbox); p.epoch = static_cast<unsigned*>(epoch); p.sums = static_cast<const float2*>(sums);
+  p.totals = static_cast<double2*>(totals);
   p.NB = NB; p.F_loc = F_loc; p.G = G; p.world = world; p.me = me;
   const int threads = std::max(64, (n + 31) / 32 * 32);
   FZ_CUDA(launch_pdl(gn_combine_kernel, dim3(1), dim3(threads), static_cast<size_t>(n) * 16, stream, p));

@@ -100,7 +100,7 @@ class UNetEngine:
     def _gn_joint(self, name: str, x3: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, F: int, silu: bool) -> torch.Tensor:
         """nn.GroupNorm over (C/G, F_total, H, W) (resnet.py:338,369; unet_3d_condition.py:439) with the frames of other ranks included:
         every rank pushes its per-image (sum, sumsq) [NB, G] into each peer's inbox (512 B .. 2 KiB over NVLink), fz_gn_combine waits for the
-        peers and folds everything into the layout the apply kernel reads."""
+        peers and folds everything, in fp64, into the layout the apply kernel reads."""
         if self.shard is None:
             return ops.groupnorm(x3, gamma, beta, eps, self.groups, F, silu, images_per_item=self._images_per_item)
         rank, world, _ = self.shard
@@ -109,10 +109,11 @@ class UNetEngine:
         nb = NB * G * 16                                                   # two 8-byte {value, epoch} words per (image, group)
         sums = ops.groupnorm_stats(x3, G)                                  # [NB, G, 2] fp32 view into the workspace
         site = ar.site(("gn", name, NB), world * nb)
+        totals = torch.empty((NB, G, 2), dtype=torch.float64, device=x3.device)
         pi = (C.c_void_p * world)(*[ar.peer_ptr(r, site, rank * nb) if r != rank else None for r in range(world)])
         _lib.call("fz_gn_combine", C.c_void_p(ar.base + site.flag_offset + 4 * 31), pi, C.c_void_p(ar.base + site.offset),
-                  C.c_void_p(sums.data_ptr()), NB, F, G, world, rank, ops._stream())
-        return ops.groupnorm_apply(x3, gamma, beta, eps, G, F, F * world, silu, sums)
+                  C.c_void_p(sums.data_ptr()), C.c_void_p(totals.data_ptr()), NB, F, G, world, rank, ops._stream())
+        return ops.groupnorm_apply(x3, gamma, beta, eps, G, F, F * world, silu, totals)
 
     def _halo_ext(self, key: tuple, y4: torch.Tensor) -> torch.Tensor:
         """y4 [B, F, HW, C] (this rank's frames) -> [B, F+2, HW, C] in the arena: interior = y4, frame 0 / F+1 = the last / first frame of the

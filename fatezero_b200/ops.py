@@ -172,13 +172,14 @@ def groupnorm_stats(x: torch.Tensor, groups: int) -> torch.Tensor:
 
 def groupnorm_apply(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, groups: int, frames_per_stat: int, count_frames: int,
                     silu: bool, sums: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Second half of the frame-sharded GroupNorm: sums [NB, groups, 2] fp32 (the apply adds frames_per_stat consecutive images)."""
+    """Second half of the frame-sharded GroupNorm: sums [NB, groups, 2] fp32 per-image sums or fp64 set totals (fz_gn_combine); the
+    apply adds frames_per_stat consecutive images in fp64."""
     _chk(x, f16, "groupnorm_apply")
     NB, HW, Cc = x.shape
-    assert x.is_contiguous() and sums.is_contiguous() and sums.dtype == torch.float32 and sums.numel() == NB * groups * 2
+    assert x.is_contiguous() and sums.is_contiguous() and sums.dtype in (torch.float32, torch.float64) and sums.numel() == NB * groups * 2
     if out is None:
         out = torch.empty_like(x)
-    _lib.call("fz_groupnorm_apply_f16", _p(x), _p(out), NB, HW, Cc, groups, frames_per_stat, count_frames, _p(gamma), _p(beta), float(eps),
+    _lib.call("fz_groupnorm_apply_sums64_f16" if sums.dtype == torch.float64 else "fz_groupnorm_apply_f16", _p(x), _p(out), NB, HW, Cc, groups, frames_per_stat, count_frames, _p(gamma), _p(beta), float(eps),
               int(silu), _p(sums), _stream())
     return out
 

@@ -162,12 +162,15 @@ int fz_groupnorm_batched_nhwc_f16(const void* x, void* y, int NB, int HW, int C,
                                   const float* gamma, const float* beta, float eps, int silu, void* workspace_f64, fz_stream_t stream);
 
 /* Frame-sharded GroupNorm (one clip's frames over several GPUs, SURVEY.md 8(e); resnet.py:338,369 normalise over ALL frames):
- * fz_groupnorm_stats_f16 leaves float2 (sum, sumsq) [NB][groups] at workspace_f64 + 768 KiB; the caller all-reduces the per-set sums over
- * the ranks (NCCL) and passes them to fz_groupnorm_apply_f16 as image_sums (the apply kernel adds frames_per_stat consecutive images of a
- * set and divides by C/groups * HW * count_frames, count_frames = frames of the set on ALL ranks). */
+ * fz_groupnorm_stats_f16 leaves float2 (sum, sumsq) [NB][groups] at workspace_f64 + 768 KiB; the caller adds the per-set sums over
+ * the ranks and passes them to fz_groupnorm_apply_f16 as image_sums, float2 (sum, sumsq) [NB][groups], or to
+ * fz_groupnorm_apply_sums64_f16 as double2 [NB][groups] (fz_gn_combine's fp64 set totals).  The apply kernel adds frames_per_stat
+ * consecutive images of a set in fp64 and divides by C/groups * HW * count_frames, count_frames = frames of the set on ALL ranks. */
 int fz_groupnorm_stats_f16(const void* x, int NB, int HW, int C, int groups, void* workspace_f64, fz_stream_t stream);
 int fz_groupnorm_apply_f16(const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, int count_frames,
                            const float* gamma, const float* beta, float eps, int silu, const void* image_sums, fz_stream_t stream);
+int fz_groupnorm_apply_sums64_f16(const void* x, void* y, int NB, int HW, int C, int groups, int frames_per_stat, int count_frames,
+                                  const float* gamma, const float* beta, float eps, int silu, const void* image_sums, fz_stream_t stream);
 /* nn.LayerNorm over channels of token rows (models/attention.py:281,303,320,331) */
 int fz_layernorm_f16(const void* x, void* y, long long M, int C, const float* gamma, const float* beta, float eps, fz_stream_t stream);
 /* F.interpolate(scale_factor=2, mode="nearest") (resnet.py:145) */
@@ -288,9 +291,10 @@ int fz_p2p_wait(void* flags, unsigned mask, fz_stream_t stream);
 /* GroupNorm statistics exchange in one single-CTA launch, low-latency protocol: every (sum, sumsq) of sums [NB*G] float2 is written into
  * peer_inbox[r] (rank r's inbox slot for this rank, [NB*G][2] 8-byte words {value, epoch}); the kernel then polls the local inbox
  * ([world][NB*G][2] words) until every peer's words carry this use's epoch (`epoch`: local per-site counter, advanced by the kernel), adds
- * them to sums and leaves each statistics set's total in the slot of its first local image (input layout of fz_groupnorm_apply_f16). */
-int fz_gn_combine(void* epoch, void* const* peer_inbox, const void* inbox, void* sums, int NB, int F_loc, int G, int world, int me,
-                  fz_stream_t stream);
+ * them to sums in fp64 and leaves each statistics set's total in the slot of its first local image of totals [NB*G] double2, 0 in the
+ * other slots (input layout of fz_groupnorm_apply_sums64_f16). */
+int fz_gn_combine(void* epoch, void* const* peer_inbox, const void* inbox, const void* sums, void* totals, int NB, int F_loc, int G, int world,
+                  int me, fz_stream_t stream);
 
 #ifdef __cplusplus
 }

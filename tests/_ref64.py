@@ -41,6 +41,10 @@ statistics of the fp16 inputs, pass when
 
 Element-wise fp32 steps (DDIM, CFG + DDIM + blend, out_temporal, the time embedding): |got - ref64| <= c * 2^-24 * sum|terms|, the
 terms being the expression evaluated on absolute values (the running-error bound of its fp32 evaluation).
+
+The GroupNorm statistics exchange of the frame-sharded forward (fz_gn_combine, test_gpu_p2p_edges.py) is checked bitwise: the fp64 total
+in the first slot of every statistics set equals an fp64 replay in the kernel's order and lies within the recursive-summation bound
+(m - 1) 2^-53 sum|v| of the exact sum of its m = world F_loc values; the other slots of the set are exactly 0.
 """
 import math
 
@@ -430,6 +434,63 @@ def quick_gelu_ref(x):
     x64 = x.double()
     ref = x64 * torch.sigmoid(f32(1.702) * x64)
     return ref, ulp16(ref) + ref.abs() * (5 + 2 * x64.abs()) * 2.0 ** -23
+
+
+# ------------------------------------------------------------------------------------------------- GroupNorm statistics exchange
+def ulp64(x: torch.Tensor) -> torch.Tensor:
+    """Spacing of fp64 numbers in the binade of |x| (2^-1074 in the subnormal range)."""
+    m, e = torch.frexp(x.double().abs().clamp(min=2.0 ** -1022))
+    return torch.ldexp(torch.ones_like(m), e - 53)
+
+
+def gn_combine_ref(own: torch.Tensor, peers: torch.Tensor, me: int, F_loc: int):
+    """fz_gn_combine in fp64.  own [NB, G, 2] fp32: this rank's per-image (sum, sumsq); peers [world, NB, G, 2] fp32: rank r's values as
+    they arrive in the inbox (row `me` unused).  Images are [B, F_loc] (a statistics set = the F_loc consecutive images of one clip item).
+    Returns (replay, exact), both [NB, G, 2] fp64 with every set's total in its first image and 0 in the others:
+      replay  the kernel's order: own value first, then the other ranks in rank order, then the frames f = 0 .. F_loc - 1;
+      exact   math.fsum over the same world * F_loc values;
+    and the sum of their absolute values (for the summation bound)."""
+    world = peers.shape[0]
+    NB, G, _ = own.shape
+    acc = own.double()
+    for r in range(world):
+        if r != me:
+            acc = acc + peers[r].double()
+    sets = acc.view(NB // F_loc, F_loc, G, 2)
+    tot = sets[:, 0]
+    for f in range(1, F_loc):
+        tot = tot + sets[:, f]
+    vals = torch.cat([own.double()[None]] + [peers[r].double()[None] for r in range(world) if r != me])  # [world, NB, G, 2]
+    vals = vals.view(world, NB // F_loc, F_loc, G, 2).permute(1, 3, 4, 0, 2).reshape(NB // F_loc, G, 2, -1)
+    exact = torch.tensor([math.fsum(v) for v in vals.reshape(-1, vals.shape[-1]).tolist()], dtype=torch.float64).view(NB // F_loc, G, 2)
+    out = [torch.zeros(NB // F_loc, F_loc, G, 2, dtype=torch.float64) for _ in range(3)]
+    out[0][:, 0], out[1][:, 0], out[2][:, 0] = tot, exact, vals.abs().sum(-1)
+    return tuple(t.view(NB, G, 2) for t in out)
+
+
+def check_gn_combine(got: torch.Tensor, own: torch.Tensor, peers: torch.Tensor, me: int, F_loc: int, report=None, key="") -> dict:
+    """got [NB, G, 2] fp64 (the totals of fz_gn_combine) against gn_combine_ref: first slots bitwise equal to the replay and within
+    (m - 1) 2^-53 sum|v| of the exact sum (m = world F_loc values), the other slots of every set exactly 0 (bitwise +0)."""
+    replay, exact, abs_sum = gn_combine_ref(own.cpu(), peers.cpu(), me, F_loc)
+    m = peers.shape[0] * F_loc
+    got = got.cpu()
+    NB, G, _ = got.shape
+    first = torch.zeros(NB // F_loc, F_loc, G, 2, dtype=torch.bool)
+    first[:, 0] = True
+    first = first.view(NB, G, 2)
+    assert got.dtype == torch.float64, got.dtype
+    gb = got.view(torch.int64)
+    bad_rest = int((gb[~first] != 0).sum().item())
+    bad_replay = int((gb[first] != replay.view(torch.int64)[first]).sum().item())
+    err = (got - exact).abs()[first]
+    ratio = err / ((m - 1) * 2.0 ** -53 * abs_sum[first]).clamp(min=1e-300)
+    stats = dict(n=got.numel(), sets=int(first.sum().item()), replay_mismatches=bad_replay, nonzero_rest=bad_rest,
+                 max_ulps_from_exact=(err / ulp64(exact[first])).max().item(), worst_err_over_bound=ratio.max().item())
+    _record(report, key, stats)
+    assert bad_rest == 0, f"{key}: {bad_rest} non-first slots of the statistics sets are not 0"
+    assert bad_replay == 0, f"{key}: {bad_replay} set totals differ from the fp64 replay in the kernel's order"
+    assert stats["worst_err_over_bound"] <= 1.0, f"{key}: a set total is off the exact sum by {stats['worst_err_over_bound']:.2f} x the summation bound"
+    return stats
 
 
 # --------------------------------------------------------------------------------------------------------- blend mask and heat maps

@@ -13,7 +13,8 @@ shared workspace: arrival counters back at zero after every        test_groupnor
   call, repeated calls bitwise equal
 fz_groupnorm_stats_f16 + fz_groupnorm_apply_f16 with count_frames  test_groupnorm_split_ranks
   > frames_per_stat (2 and 4 emulated ranks), batched GroupNorm    test_groupnorm_batched
-  at K = 8 items
+  at K = 8 items; fz_groupnorm_apply_sums64_f16 with fp64 set     test_groupnorm_apply_fp64_sums
+  totals that fp32 cannot hold (constant groups, 12 frames)
 mean / sigma in {0, 4, 16, 64, 256}, constant and near-constant     test_groupnorm_dc_offset, test_layernorm_dc_offset,
   groups and rows (the fused-shift and E[x^2] - mu^2 paths);         test_groupnorm_constant_groups
   constant groups with SiLU, 2 slots, split statistics + apply
@@ -224,6 +225,26 @@ def test_groupnorm_constant_groups(C, report):
     stats = [ops.groupnorm_stats(p, G).clone() for p in parts]
     outs = [ops.groupnorm_apply(p, g, b, 1e-5, G, 2, NB, False, stats[0] + stats[1]) for p in parts]
     gn_check(torch.cat(outs), x, g, b, 1e-5, G, NB, False, report, f"gn_const_C{C}_split")
+
+
+@pytest.mark.parametrize("silu", [False, True])
+def test_groupnorm_apply_fp64_sums(silu, report):
+    """The apply of the frame-sharded GroupNorm with fp64 set totals (what fz_gn_combine leaves): constant groups of 0.3 (fp16 1229 / 4096)
+    over C / G * HW * F = 10 * 1023 * 12 elements, whose per-image sums are exact in fp32 but whose set total needs more than 24 bits.
+    Four emulated ranks of 3 frames each; the total sits in the first image of each set, the other images hold 0.  Strict bound."""
+    B, Fr, HW, C, G, R = 2, 12, 1023, 320, 32, 4
+    Fl = Fr // R
+    x = dc_input((B, Fr, HW, G, C // G), "const", 57, (1, 1, 1, G, 1)).reshape(B, Fr, HW, C).half()
+    g, b = affine(C, 58)
+    b = b * 0.05
+    parts = [x[:, r * Fl:(r + 1) * Fl].reshape(B * Fl, HW, C).contiguous() for r in range(R)]
+    stats = [ops.groupnorm_stats(p, G).double().view(B, Fl, G, 2) for p in parts]
+    totals = torch.zeros(B, Fl, G, 2, dtype=torch.float64, device=dev)
+    totals[:, 0] = sum(s.sum(1) for s in stats)
+    outs = [ops.groupnorm_apply(p, g, b, 1e-5, G, Fl, Fr, silu, totals.view(B * Fl, G, 2)) for p in parts]
+    got = torch.stack([o.view(B, Fl, HW, C) for o in outs], 1).reshape(B * Fr, HW, C)
+    assert totals[:, 0].float().double().ne(totals[:, 0]).any(), "no set total is inexact in fp32: the case no longer tests fp64 sums"
+    gn_check(got, x.reshape(B * Fr, HW, C), g, b, 1e-5, G, Fr, silu, report, f"gn_apply_fp64_silu{int(silu)}")
 
 
 @pytest.mark.parametrize("mode", DC_CASES, ids=str)

@@ -3,14 +3,15 @@ result with one element moved by 3 ulps, a bias applied one column off, or one 6
 normalised slightly differently or one 64-key block missing).  The norm bounds reject a variance over n - 1, eps outside the square root,
 per-frame instead of joint-frame statistics and the fused-shift rounding on a constant row; the softmax bound a scale one fp16 ulp off;
 the mask and heat-map checks a resize index off by one (and the integer nearest index) and a white all-zero column; the step bound CFG
-guidance applied to the wrong half.  No GPU: everything here is fp64 on the CPU."""
+guidance applied to the wrong half.  The GroupNorm statistics-exchange check rejects sets read as [F_loc, B], the own rank counted twice,
+non-first slots left unzeroed and a rounding to fp32 after every rank's add (or of the set total).  No GPU: everything here is fp64 on the CPU."""
 import pytest
 import torch
 import torch.nn.functional as F
 
 from _ref64 import (X_A, X_ALPHA, X_EQ, X_M, X_MAP, blend_mask_ratio, cfg_ddim_ref, check_attn, check_edit, check_heatmaps, check_mask,
-                    check_probs, check_running_sum, check_step, check_tap, cross_edit_ref, cross_edit_table, ddim_invert_ref, gemm_ref, gn_check,
-                    heatmap_values, ln_check, nearest_index, softmax64, ulp16)
+                    check_gn_combine, check_probs, check_running_sum, check_step, check_tap, cross_edit_ref, cross_edit_table, ddim_invert_ref,
+                    gemm_ref, gn_check, heatmap_values, ln_check, nearest_index, softmax64, ulp16)
 
 
 def rnd(*shape, seed=0, scale=1.0):
@@ -353,3 +354,59 @@ def test_step_rejects_guidance_on_wrong_half():
         check_step(wrong.float(), ref, terms)
     inv, inv_terms = ddim_invert_ref(x, eps2[:K], 0.3, 0.4)
     check_step(inv.float(), inv, inv_terms)
+
+
+# ---------------------------------------------------------------------------------------------------- GroupNorm statistics exchange
+def combine_case(world=4, me=1, B=3, F_loc=4, G=5, seed=100):
+    """Per-image (sum, sumsq) of every rank with magnitudes spread over 2^-12 .. 2^12, so that any change of the fold order or of the
+    rounding points moves some totals."""
+    g = torch.Generator().manual_seed(seed)
+    v = torch.randn(world, B * F_loc, G, 2, generator=g) * torch.pow(2.0, torch.randint(-12, 13, (world, B * F_loc, G, 2), generator=g).float())
+    v[..., 1] = v[..., 1].abs()
+    return v[me].clone(), v
+
+
+def fold64(acc, F_loc, sets_minor=True, zero_rest=True):
+    """Fold the fp64 per-image totals acc [NB, G, 2] over the frames of each set; sets_minor=False reads the images as [F_loc, B]."""
+    NB, G, _ = acc.shape
+    v = acc.view(NB // F_loc, F_loc, G, 2) if sets_minor else acc.view(F_loc, NB // F_loc, G, 2).transpose(0, 1)
+    tot = v[:, 0]
+    for f in range(1, F_loc):
+        tot = tot + v[:, f]
+    out = torch.zeros(NB // F_loc, F_loc, G, 2, dtype=torch.float64) if zero_rest else acc.view(NB // F_loc, F_loc, G, 2).clone()
+    out[:, 0] = tot
+    return out.view(NB, G, 2)
+
+
+def rank_sum(own, peers, me, own_times=1, round_each=False):
+    acc = own.double() * own_times
+    for r in range(peers.shape[0]):
+        if r != me:
+            acc = acc + peers[r].double()
+            if round_each:
+                acc = acc.float().double()
+    return acc
+
+
+def test_gn_combine_accepts_kernel_order():
+    for world, me, F_loc in [(4, 1, 4), (1, 0, 2), (3, 2, 1)]:
+        own, peers = combine_case(world, me, F_loc=F_loc)
+        check_gn_combine(fold64(rank_sum(own, peers, me), F_loc), own, peers, me, F_loc)
+
+
+@pytest.mark.parametrize("bug", ["sets_as_F_by_B", "own_rank_twice", "rest_not_zeroed", "per_rank_fp32_rounding", "fp32_set_total"])
+def test_gn_combine_rejects(bug):
+    own, peers = combine_case()
+    me, F_loc = 1, 4
+    if bug == "sets_as_F_by_B":
+        got = fold64(rank_sum(own, peers, me), F_loc, sets_minor=False)
+    elif bug == "own_rank_twice":
+        got = fold64(rank_sum(own, peers, me, own_times=2), F_loc)
+    elif bug == "rest_not_zeroed":
+        got = fold64(rank_sum(own, peers, me), F_loc, zero_rest=False)
+    elif bug == "per_rank_fp32_rounding":
+        got = fold64(rank_sum(own, peers, me, round_each=True), F_loc)
+    else:
+        got = fold64(rank_sum(own, peers, me), F_loc).float().double()
+    with pytest.raises(AssertionError, match="are not 0" if bug == "rest_not_zeroed" else "differ from the fp64 replay"):
+        check_gn_combine(got, own, peers, me, F_loc)
