@@ -484,11 +484,14 @@ static int conv3x3_impl(const void* x, long long ldx, int NB, int H, int W, int 
   FZ_CHECK_ARG(Cin % 8 == 0 && ldx % 8 == 0, "fz_conv3x3: Cin/ldx must be multiples of 8");
   FZ_CHECK_ARG(stride == 1 || (H % 2 == 0 && W % 2 == 0), "fz_conv3x3: stride 2 needs even H, W");
   const int Ho = H / stride, Wo = W / stride;
-  FZ_CHECK_ARG(Wo <= 128 || Wo % 128 == 0, "fz_conv3x3: output width %d must be <= 128 or a multiple of 128", Wo);
   FZ_CHECK_ARG(!asym_pad || stride == 2, "fz_conv3x3: asymmetric padding is the stride-2 downsample variant");
-  // box over (x, y, n): the full output width (or 128-pixel row segments of wider images: VAE resolutions), as many rows / images as fit
-  // 128 GEMM rows
-  int bw = std::min(Wo, 128), bh = (bw == Wo) ? std::min(Ho, 128 / bw) : 1;
+  // box over (x, y, n): the full output width, as many rows / images as fit 128 GEMM rows.  Wider images (VAE resolutions) are tiled in
+  // row segments of bw pixels, bw the largest divisor of Wo up to 128 (Wo 256, 512: 128; 192, 288, 576: 96; 144: 72; 160, 320: 80), so a
+  // tile never crosses an image row
+  int bw = std::min(Wo, 128);
+  while (Wo % bw) --bw;
+  FZ_CHECK_ARG(Wo <= 128 || bw >= 8, "fz_conv3x3: output width %d has no divisor in [8, 128] to tile its rows with", Wo);
+  int bh = (bw == Wo) ? std::min(Ho, 128 / bw) : 1;
   while (Ho % bh) --bh;
   int bn_img = (bh == Ho) ? std::min(NB, 128 / (bw * bh)) : 1;
   while (NB % bn_img) --bn_img;

@@ -90,7 +90,9 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias=None, residual=None, out=None, g
 
 def conv3x3(x: torch.Tensor, w9: torch.Tensor, bias=None, stride: int = 1, residual=None, group_bias=None, rows_per_group=0,
             force_bn: int = 0, asym_pad: bool = False) -> torch.Tensor:
-    """x [NB,H,W,Cin] fp16 NHWC, w9 [9,Cout,Cin] -> [NB,H/stride,W/stride,Cout].  asym_pad (stride 2): right/bottom-only padding."""
+    """x [NB,H,W,Cin] fp16 NHWC, w9 [9,Cout,Cin] -> [NB,H/stride,W/stride,Cout].  asym_pad (stride 2): right/bottom-only padding.
+    Output widths above 128 are tiled in row segments of the largest divisor of the width up to 128; a width whose largest such divisor
+    is below 8 (e.g. 262 = 2 x 131) is refused."""
     _chk(x, f16, "conv3x3"); _chk(w9, f16, "conv3x3")
     NB, H, W, Cin = x.shape
     Cout = w9.shape[1]

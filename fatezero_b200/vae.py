@@ -4,8 +4,9 @@
 
 `VaeEngine` executes the SD-1.x VAE (diffusers 0.11.1 `AutoencoderKL`: DownEncoderBlock2D / UNetMidBlock2D with a single-head 512-wide
 AttentionBlock / UpDecoderBlock2D, GroupNorm(32, eps 1e-6) + SiLU, no time embedding) with the kernels of libfatezero_b200.so:
-  * every 3x3 conv is the tap-GEMM (`fz_conv3x3_nhwc_f16`; images wider than 128 pixels are tiled in 128-pixel row segments; the encoder's
-    downsample is the right/bottom-padded stride-2 variant `fz_conv3x3_down_asym_nhwc_f16`), 1x1 shortcuts and attention projections are
+  * every 3x3 conv is the tap-GEMM (`fz_conv3x3_nhwc_f16`; images wider than 128 pixels are tiled in row segments whose width is the
+    largest divisor of the output width up to 128: 128 at 256 / 512 / 640 / 768, 96 at 192 / 288 / 576, 80 at 160 / 320, 72 at 144;
+    the encoder's downsample is the right/bottom-padded stride-2 variant `fz_conv3x3_down_asym_nhwc_f16`), 1x1 shortcuts and attention projections are
     `fz_gemm_f16`, the RGB / latent input convs go through the im2col GEMM like the UNet's conv_in;
   * GroupNorm(+SiLU), nearest upsampling: the UNet's HBM-bound kernels;
   * the mid-block attention (one head of width 512: more than the fused attention kernel holds in registers) runs per image as
@@ -14,8 +15,9 @@ AttentionBlock / UpDecoderBlock2D, GroupNorm(32, eps 1e-6) + SiLU, no time embed
 fp16 storage / fp32 accumulation, fp32 in and out.  `AutoencoderKL` below is a parameter container with the diffusers state-dict names and
 the `encode(...).latent_dist.sample(generator)` / `decode(...).sample` surface, so it can be handed to the pipeline as `vae`; the pipeline
 also wraps a foreign AutoencoderKL-shaped module (diffusers) that lives on the GPU (`pipeline._vae()`).
-Numerics are checked against an fp32 torch restatement (oracle/vae_oracle.py, tests/test_gpu_vae.py); that restatement is NOT pinned to
-the real diffusers package (absent offline) — see DESIGN.md §5."""
+Numerics are checked against an fp32 torch restatement (oracle/vae_oracle.py, tests/test_gpu_vae.py), every kernel call of encode / decode
+against fp64 at 512 and 768 pixels and every block against an independent fp64 restatement (tests/test_gpu_vae_blocks.py); neither
+restatement is pinned to the real diffusers package (absent offline) — see DESIGN.md §5."""
 from __future__ import annotations
 
 import math
@@ -221,39 +223,54 @@ class VaeEngine:
         cols = ops.im2col_latents(x_nchw.to(f32).permute(1, 0, 2, 3)[None].contiguous())    # [N*H*W, 64]
         return ops.gemm(cols, self.w[name + ".weight"], bias=self.w[name + ".bias"]).view(N, H, W, -1)
 
+    def _down(self, n: str, x: torch.Tensor) -> torch.Tensor:  # Downsample2D(padding=0): F.pad(x, (0, 1, 0, 1)), 3x3 conv stride 2
+        return ops.conv3x3(x, self.w[n + ".conv.weight"], bias=self.w[n + ".conv.bias"], stride=2, asym_pad=True)
+
+    def _up(self, n: str, x: torch.Tensor) -> torch.Tensor:  # Upsample2D: nearest 2x, 3x3 conv
+        return ops.conv3x3(ops.upsample2x(x), self.w[n + ".conv.weight"], bias=self.w[n + ".conv.bias"])
+
+    def _encoder_out(self, x: torch.Tensor) -> torch.Tensor:
+        """conv_norm_out + SiLU + conv_out with quant_conv folded in -> moments [N, 2*latent, H, W] fp32."""
+        w = self.w
+        y = ops.conv3x3(self._gn("encoder.conv_norm_out", x, True), w["encoder.conv_out.weight"], bias=w["encoder.conv_out.bias"])
+        return y[..., : 2 * self.lat].permute(0, 3, 1, 2).float().contiguous()
+
+    def _decoder_in(self, z: torch.Tensor) -> torch.Tensor:
+        """post_quant_conv (4x4 per pixel, fp32) + decoder conv_in: latents [N, latent, h, w] -> [N, h, w, C] fp16."""
+        w = self.w
+        z = torch.einsum("oc,nchw->nohw", w["post_quant_conv.weight"], z.to(self.dev, f32)) + w["post_quant_conv.bias"][None, :, None, None]
+        return self._conv_in("decoder.conv_in", z)
+
+    def _decoder_out(self, x: torch.Tensor) -> torch.Tensor:
+        """conv_norm_out + SiLU + conv_out -> images [N, 3, H, W] fp32."""
+        w = self.w
+        y = ops.conv3x3(self._gn("decoder.conv_norm_out", x, True), w["decoder.conv_out.weight"], bias=w["decoder.conv_out.bias"])
+        return y[..., : self.cfg["out_channels"]].permute(0, 3, 1, 2).float().contiguous()
+
     # ---- public ---------------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def encode_moments(self, images: torch.Tensor) -> torch.Tensor:
         """images [N, 3, H, W] (CUDA, any float dtype, values in [-1, 1]) -> moments [N, 2*latent, H/8, W/8] fp32 (mean | logvar)."""
-        w = self.w
         with torch.cuda.device(self.dev):
             x = self._conv_in("encoder.conv_in", images.to(self.dev))
             for i in range(len(self.ch)):
                 for j in range(self.lpb):
                     x = self._resnet(f"encoder.down_blocks.{i}.resnets.{j}", x)
                 if i != len(self.ch) - 1:
-                    d = f"encoder.down_blocks.{i}.downsamplers.0.conv"
-                    x = ops.conv3x3(x, w[d + ".weight"], bias=w[d + ".bias"], stride=2, asym_pad=True)
-            x = self._mid("encoder.mid_block", x)
-            y = ops.conv3x3(self._gn("encoder.conv_norm_out", x, True), w["encoder.conv_out.weight"], bias=w["encoder.conv_out.bias"])
-            return y[..., : 2 * self.lat].permute(0, 3, 1, 2).float().contiguous()
+                    x = self._down(f"encoder.down_blocks.{i}.downsamplers.0", x)
+            return self._encoder_out(self._mid("encoder.mid_block", x))
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor) -> torch.Tensor:
         """latents [N, latent, h, w] (already divided by the 0.18215 scaling factor by the caller) -> images [N, 3, 8h, 8w] fp32."""
-        w = self.w
         with torch.cuda.device(self.dev):
-            z = z.to(self.dev, f32)
-            z = torch.einsum("oc,nchw->nohw", w["post_quant_conv.weight"], z) + w["post_quant_conv.bias"][None, :, None, None]  # 4x4 per pixel
-            x = self._mid("decoder.mid_block", self._conv_in("decoder.conv_in", z))
+            x = self._mid("decoder.mid_block", self._decoder_in(z))
             for i in range(len(self.ch)):
                 for j in range(self.lpb + 1):
                     x = self._resnet(f"decoder.up_blocks.{i}.resnets.{j}", x)
                 if i != len(self.ch) - 1:
-                    u = f"decoder.up_blocks.{i}.upsamplers.0.conv"
-                    x = ops.conv3x3(ops.upsample2x(x), w[u + ".weight"], bias=w[u + ".bias"])
-            y = ops.conv3x3(self._gn("decoder.conv_norm_out", x, True), w["decoder.conv_out.weight"], bias=w["decoder.conv_out.bias"])
-            return y[..., : self.cfg["out_channels"]].permute(0, 3, 1, 2).float().contiguous()
+                    x = self._up(f"decoder.up_blocks.{i}.upsamplers.0", x)
+            return self._decoder_out(x)
 
 
 class _Config(dict):

@@ -42,6 +42,12 @@ statistics of the fp16 inputs, pass when
 Element-wise fp32 steps (DDIM, CFG + DDIM + blend, out_temporal, the time embedding): |got - ref64| <= c * 2^-24 * sum|terms|, the
 terms being the expression evaluated on absolute values (the running-error bound of its fp32 evaluation).
 
+VAE blocks (test_gpu_vae_blocks.py) are checked against VaeBlocks64, an fp64 restatement of the diffusers 0.11.1 AutoencoderKL blocks,
+on the fp16 floor: the same restatement run in torch fp16 on the GPU (weights in half, as the reference's fp16 pipeline runs them) deviates
+from fp64 by floor = max|o16 - ref64|; the engine's block passes when
+
+    max|got - ref64| <= 1.5 floor + 2 ulp16(max|ref64|)
+
 The GroupNorm statistics exchange of the frame-sharded forward (fz_gn_combine, test_gpu_p2p_edges.py) is checked bitwise: the fp64 total
 in the first slot of every statistics set equals an fp64 replay in the kernel's order and lies within the recursive-summation bound
 (m - 1) 2^-53 sum|v| of the exact sum of its m = world F_loc values; the other slots of the set are exactly 0.
@@ -135,6 +141,21 @@ def conv3x3_ref(x, w9, stride=1, asym_pad=False, **epi):
         return F.conv2d(xx, ww, stride=stride, padding=pad).permute(0, 2, 3, 1).reshape(-1, Cout)
 
     return epilogue_ref(conv(x64, w64), conv(x64.abs(), w64.abs()), **epi)
+
+
+def conv3x3_rows_ref(x, w9, rows, stride=1, asym_pad=False, **epi):
+    """conv3x3_ref on the output rows `rows` (flat indices into [NB, Ho, Wo]) only: the 9 input pixels of each row are gathered, so the
+    fp64 work scales with len(rows), not with the image.  -> (ref, sum|terms|) [len(rows), Cout] fp64; epilogue tensors already row-selected."""
+    NB, H, W, Cin = x.shape
+    Ho, Wo = H // stride, W // stride
+    # output (y, x) reads input row stride y + ky - 1 (symmetric) or stride y + ky (right/bottom padding): index stride y + ky of xp
+    xp = F.pad(x, (0, 0, 0, 1, 0, 1)) if asym_pad else F.pad(x, (0, 0, 1, 1, 1, 1))
+    rows = rows.to(x.device)
+    n, r = rows // (Ho * Wo), rows % (Ho * Wo)
+    yy, xx = r // Wo, r % Wo
+    a = torch.stack([xp[n, stride * yy + ky, stride * xx + kx] for ky in range(3) for kx in range(3)], 1).double()  # [R, 9, Cin]
+    w64 = w9.double()
+    return epilogue_ref(torch.einsum("rtc,toc->ro", a, w64), torch.einsum("rtc,toc->ro", a.abs(), w64.abs()), **epi)
 
 
 def tconv3_ref(x, w3, halo=False, **epi):
@@ -545,4 +566,141 @@ def check_heatmaps(got, v, report=None, key="") -> dict:
     stats = dict(n=got.numel(), n_near=int(near.sum().item()), mismatches=int(bad.sum().item()))
     _record(report, key, stats)
     assert stats["mismatches"] == 0, f"{key}: {stats['mismatches']} heat-map pixels differ from the fp64 reference ({stats})"
+    return stats
+
+
+# ---------------------------------------------------------------------------------------------------------------------------- VAE blocks
+class VaeBlocks64:
+    """The blocks of diffusers 0.11.1 AutoencoderKL, NCHW, restated from the published forward code of that release (models/resnet.py
+    ResnetBlock2D / Downsample2D(padding=0) / Upsample2D, models/attention.py AttentionBlock, models/vae.py Encoder / Decoder heads,
+    AutoencoderKL quant_conv / post_quant_conv), independently of oracle/vae_oracle.py.
+
+    It computes in the dtype it is given: float64 for the reference; float16 on the GPU for the fp16 floor (weights in half, the attention
+    scores through baddbmm with alpha = scale and the softmax in fp32 cast back to half, as AttentionBlock runs under fp16).  `rnd` is
+    applied to the result of every op: identity, or a rounding to fp16 to emulate the fp16 run in fp64 on the CPU.  `bug` selects one
+    deliberate mistake from BUGS (test_ref64_selfcheck.py shows that check_block rejects each)."""
+    BUGS = ("qk_swapped", "scale_1_over_c", "scale_c_quarter", "softmax_over_queries", "vbias_dropped", "vbias_unnormalised",
+            "quant_wq_transposed", "conv_out_col_offset", "down_pad_left_top", "gn_eps_1e-5", "upsample_index_off_by_one")
+
+    def __init__(self, sd, dtype, device, groups: int = 32, rnd=None, bug=None):
+        assert bug is None or bug in self.BUGS, bug
+        self.sd, self.dtype, self.dev, self.groups = sd, dtype, device, groups
+        self.rnd = rnd or (lambda t: t)
+        self.bug = bug
+
+    def p(self, name):
+        return self.sd[name].to(self.dev, self.dtype)
+
+    def conv(self, n, x, stride=1, padding=1):
+        return self.rnd(F.conv2d(x, self.p(n + ".weight"), self.p(n + ".bias"), stride=stride, padding=padding))
+
+    def gn(self, n, x, silu):
+        eps = 1e-5 if self.bug == "gn_eps_1e-5" else 1e-6
+        y = self.rnd(F.group_norm(x, self.groups, self.p(n + ".weight"), self.p(n + ".bias"), eps))
+        return self.rnd(F.silu(y)) if silu else y
+
+    def resnet(self, n, x):
+        h = self.conv(n + ".conv1", self.gn(n + ".norm1", x, True))
+        h = self.conv(n + ".conv2", self.gn(n + ".norm2", h, True))
+        if n + ".conv_shortcut.weight" in self.sd:
+            x = self.conv(n + ".conv_shortcut", x, padding=0)
+        return self.rnd(x + h)  # output_scale_factor 1
+
+    def attn(self, n, x, probs_out=None):
+        """AttentionBlock (one head of width C, rescale_output_factor 1).  probs_out: a list that receives the probabilities."""
+        B, Cc, H, W = x.shape
+        h = self.gn(n + ".group_norm", x, False).reshape(B, Cc, H * W).transpose(1, 2)
+        q = self.rnd(F.linear(h, self.p(n + ".query.weight"), self.p(n + ".query.bias")))
+        k = self.rnd(F.linear(h, self.p(n + ".key.weight"), self.p(n + ".key.bias")))
+        bv = self.p(n + ".value.bias")
+        v = self.rnd(F.linear(h, self.p(n + ".value.weight"), None if self.bug in ("vbias_dropped", "vbias_unnormalised") else bv))
+        if self.bug == "qk_swapped":
+            q, k = k, q
+        scale = {"scale_1_over_c": 1.0 / Cc, "scale_c_quarter": Cc ** -0.25}.get(self.bug, Cc ** -0.5)
+        s = self.rnd(torch.baddbmm(torch.empty(B, H * W, H * W, dtype=q.dtype, device=q.device), q, k.transpose(1, 2), beta=0, alpha=scale))
+        dim = -2 if self.bug == "softmax_over_queries" else -1
+        pr = self.rnd(torch.softmax(s.float() if s.dtype == torch.float16 else s, dim=dim).to(s.dtype))
+        if probs_out is not None:
+            probs_out.append(pr)
+        o = self.rnd(torch.bmm(pr, v))
+        if self.bug == "vbias_unnormalised":
+            # the bias rides through the un-normalised exp(s - max): it comes out multiplied by the row sum instead of by 1
+            e = torch.exp(s.double() - s.double().amax(-1, keepdim=True)).sum(-1, keepdim=True).to(o.dtype)
+            o = self.rnd(o + e * bv)
+        o = self.rnd(F.linear(o, self.p(n + ".proj_attn.weight"), self.p(n + ".proj_attn.bias")))
+        return self.rnd(o.transpose(1, 2).reshape(B, Cc, H, W) + x)
+
+    def down(self, n, x):
+        pad = (1, 0, 1, 0) if self.bug == "down_pad_left_top" else (0, 1, 0, 1)
+        return self.conv(n + ".conv", F.pad(x, pad), stride=2, padding=0)
+
+    def up(self, n, x):
+        H, W = x.shape[-2:]
+        if self.bug == "upsample_index_off_by_one":
+            iy, ix = ((torch.arange(2 * H) + 1) // 2).clamp(max=H - 1), ((torch.arange(2 * W) + 1) // 2).clamp(max=W - 1)
+            x = x[:, :, iy.to(x.device)][:, :, :, ix.to(x.device)]
+        else:
+            x = F.interpolate(x, scale_factor=2.0, mode="nearest")
+        return self.conv(n + ".conv", x)
+
+    def _col_offset(self, y):  # the conv_out's padded output read one column late: channel c from column c + 1 (the last from a zero pad)
+        return torch.cat([y[:, 1:], torch.zeros_like(y[:, :1])], 1) if self.bug == "conv_out_col_offset" else y
+
+    def encoder_in(self, img):
+        return self.conv("encoder.conv_in", img)
+
+    def encoder_out(self, x):
+        """conv_norm_out + SiLU + conv_out + quant_conv -> moments (mean | logvar)."""
+        h = self.conv("encoder.conv_out", self.gn("encoder.conv_norm_out", x, True))
+        wq = self.p("quant_conv.weight")
+        if self.bug == "quant_wq_transposed":
+            wq = wq.transpose(0, 1)
+        return self._col_offset(self.rnd(F.conv2d(h, wq, self.p("quant_conv.bias"))))
+
+    def decoder_in(self, z):
+        return self.conv("decoder.conv_in", self.conv("post_quant_conv", z, padding=0))
+
+    def decoder_out(self, x):
+        return self._col_offset(self.conv("decoder.conv_out", self.gn("decoder.conv_norm_out", x, True)))
+
+
+def vae_block_state_dict(spec, seed: int = 0, qk_scale: float = 3.0):
+    """Seeded fp32 AutoencoderKL weights {name: shape} -> {name: tensor} whose blocks are sensitive to the mistakes check_block must catch:
+    biases of std 0.3 (the value bias is visible after P V), and query / key weights scaled by qk_scale over the fan_in^-1/2 default, so
+    that the single-head attention over a GroupNorm'ed input is peaked (median row maximum ~0.7 at 4096 keys for qk_scale 3) instead of
+    close to uniform."""
+    sd = {}
+    for i, name in enumerate(sorted(spec)):
+        shape = tuple(spec[name])
+        g = torch.Generator().manual_seed(seed * 100003 + i)
+        t = torch.randn(shape, generator=g)
+        if name.endswith("bias"):
+            t = 0.3 * t
+        elif len(shape) == 1:
+            t = 1 + 0.2 * t
+        else:
+            t = t * math.prod(shape[1:]) ** -0.5
+            if ".attentions.0.query." in name or ".attentions.0.key." in name:
+                t = t * qk_scale
+        sd[name] = t
+    return sd
+
+
+FLOOR_RATIO = 1.5  # the engine may deviate from fp64 1.5 times as much as the fp16 restatement does, plus K_ULP_BLOCK fp16 ulps
+K_ULP_BLOCK = 2.0
+
+
+def check_block(got, ref, o16, report=None, key="") -> dict:
+    """A VAE block's output against its fp64 restatement on the fp16 floor (module docstring): got, ref, o16 of one shape."""
+    got, ref, o16 = got.double(), ref.double(), o16.double()
+    assert got.shape == ref.shape == o16.shape, (got.shape, ref.shape, o16.shape)
+    assert torch.isfinite(got).all(), f"{key}: non-finite output"
+    err = (got - ref).abs()
+    floor = (o16 - ref).abs().max().item()
+    bound = FLOOR_RATIO * floor + K_ULP_BLOCK * ulp16(ref.abs().max()).item()
+    stats = dict(max_abs=err.max().item(), fp16_floor=floor, ratio_to_floor=err.max().item() / max(floor, 1e-300), bound=bound,
+                 max_ulps=(err / ulp16(ref)).max().item(), ref_abs_max=ref.abs().max().item(), n=ref.numel())
+    _record(report, key, stats)
+    assert stats["max_abs"] <= bound, (f"{key}: max|got - ref64| {stats['max_abs']:.4g} > {FLOOR_RATIO} x fp16 floor {floor:.4g} + "
+                                       f"{K_ULP_BLOCK:g} ulps = {bound:.4g}")
     return stats

@@ -250,17 +250,19 @@ def test_blend_mask(report):
         assert frac < 2e-3  # ties at the threshold can flip with summation order
 
 
-def test_limits_conv_width_and_groupnorm_batch(report):
-    """Hard limits of the C ABI with a test AT the limit and an error beyond it: 3x3 conv output width 128 (one TMA box row), GroupNorm over
-    256 images with 64 groups (the 1 MiB workspace)."""
-    x = rnd(1, 8, 128, 64).half()
+def test_limits_conv_row_segments_and_groupnorm_batch(report):
+    """Hard limits of the C ABI with a test AT the limit and an error beyond it: 3x3 conv output width 128 (one TMA box row), wider rows
+    tiled in segments of their largest divisor up to 128 (136: two 68-pixel segments), a width without such a divisor of at least 8
+    refused (262 = 2 x 131); GroupNorm over 256 images with 64 groups (the 1 MiB workspace)."""
     w = rnd(64, 64, 3, 3, scale=(64 * 9) ** -0.5, seed=1)
     w9 = w.permute(2, 3, 0, 1).reshape(9, 64, 64).half().contiguous()
-    out = ops.conv3x3(x, w9)
-    ref = F.conv2d(x.float().permute(0, 3, 1, 2), w9.float().reshape(3, 3, 64, 64).permute(2, 3, 0, 1), padding=1).permute(0, 2, 3, 1)
-    close(out, ref, report, "conv_w128", atol=2e-2, rtol=2e-3)
+    for width in (128, 136):
+        x = rnd(1, 8, width, 64).half()
+        out = ops.conv3x3(x, w9)
+        ref = F.conv2d(x.float().permute(0, 3, 1, 2), w9.float().reshape(3, 3, 64, 64).permute(2, 3, 0, 1), padding=1).permute(0, 2, 3, 1)
+        close(out, ref, report, f"conv_w{width}", atol=2e-2, rtol=2e-3)
     with pytest.raises(RuntimeError, match="width"):
-        ops.conv3x3(rnd(1, 8, 136, 64).half(), w9)
+        ops.conv3x3(rnd(1, 8, 262, 64).half(), w9)
     xg = rnd(256, 16, 128).half()
     g, b = 1 + 0.1 * rnd(128, seed=3), 0.1 * rnd(128, seed=4)
     y = ops.groupnorm(xg, g, b, 1e-5, 64, 1, False)

@@ -16,11 +16,15 @@ V^T epilogue: vt_ld > S, bias on V columns, tiles spanning two      test_gemm_vt
 GEGLU at every packed width (BLOCK_N 256, 160, 128, 64, 32)        test_geglu
 GEGLU + residual / group_bias / V^T refused on the host             test_geglu_refuses_other_terms
 conv3x3 s1: 25-row tile (warpgroup 1 idle), Ho % bh adjustment,     test_conv3x3_s1
-  several images per tile, 64x96, 256-wide row segments,
-  Cin in {8, 72, 320}, every BLOCK_N, bias + group_bias + residual
+  several images per tile, 64x96, 128-pixel row segments (W 256),
+  96- and 80-pixel row segments (W 192, 320, 576: VAE widths that
+  are not multiples of 128), Cin in {8, 72, 320}, every BLOCK_N,
+  bias + group_bias + residual
 conv3x3 s2: symmetric and asymmetric (VAE downsample) padding,      test_conv3x3_s2
   odd output size, Cin not a multiple of 64 (c0 walks into the
-  next pixel's channels, cancelled by the zero-filled W columns)
+  next pixel's channels, cancelled by the zero-filled W columns),
+  256-, 192- and 288-wide outputs (128- and 96-pixel segments)
+output widths without a divisor in [8, 128] refused on the host     test_conv3x3_refuses_width
 tconv3: F in {1, 2, 3, 5, 16, 24}, several frames per tile with     test_tconv3
   F % bf adjustment, 100-pixel box (HW 200), 1-row tiles (HW 131),
   bias + residual + residual2 + group_bias (the LoRA path)
@@ -231,6 +235,10 @@ CONV_S1 = [
     (6, 4, 4, 320, 96, 128),   # 6 images per tile (96 rows)
     (1, 64, 96, 8, 64, 64),    # non-square, one 96-pixel row per tile
     (1, 3, 256, 72, 48, 32),   # 256-wide: two 128-pixel row segments per image row
+    (1, 3, 192, 72, 40, 64),   # 192-wide (VAE at 768: encoder level 2, decoder level 0): two 96-pixel segments
+    (2, 2, 320, 8, 48, 160),   # 320-wide (VAE at 640): four 80-pixel segments, two images
+    (1, 2, 576, 32, 24, 16),   # 576-wide (VAE at 576): six 96-pixel segments
+    (1, 4, 192, 320, 160, 256),  # 192-wide at Cin 320: 5 k-blocks per tap
 ]
 
 
@@ -255,6 +263,11 @@ CONV_S2 = [
     (1, 32, 32, 32, 160, 160, False),
     (1, 4, 512, 32, 33, 32, True),    # 256-wide output (VAE resolutions), odd Cout
     (2, 10, 10, 72, 256, 256, False),
+    (1, 4, 384, 32, 40, 32, True),    # 192-wide output (the VAE encoder's second downsample at 768): 96-pixel segments
+    (2, 4, 384, 72, 64, 128, False),  # the same width, symmetric padding
+    (1, 6, 576, 8, 24, 256, True),    # 288-wide output (VAE at 576), three output rows
+    (1, 2, 576, 32, 160, 160, False),
+    (1, 4, 384, 72, 24, 16, True),
 ]
 
 
@@ -266,6 +279,17 @@ def test_conv3x3_s2(NB, H, W, Cin, Cout, bn, asym, report):
     got = twice(lambda: ops.conv3x3(x, w9, bias=bias, stride=2, residual=res, force_bn=bn, asym_pad=asym))
     ref, terms = conv3x3_ref(x, w9, stride=2, asym_pad=asym, bias=bias, residuals=(res,))
     check_tap(got.reshape(-1, Cout), ref, terms, 9 * Cin + 2, report, f"conv_s2_{'asym' if asym else 'sym'}_{NB}x{H}x{W}x{Cin}->{Cout}_bn{bn}")
+
+
+@pytest.mark.parametrize("W,stride,asym", [(262, 1, False), (524, 2, True), (524, 2, False), (131 * 3, 1, False)])
+def test_conv3x3_refuses_width(W, stride, asym):
+    """An output width above 128 whose largest divisor up to 128 is below 8 (262 = 2 x 131, 393 = 3 x 131) would need 1- to 3-row tiles:
+    refused before launch, whatever the stride."""
+    Wo = W // stride
+    x, w9 = conv_inputs(1, 2 * stride, W, 8, 16, seed=75)
+    with pytest.raises(RuntimeError, match=f"output width {Wo} has no divisor"):
+        ops.conv3x3(x, w9, stride=stride, asym_pad=asym, force_bn=16)
+    torch.cuda.synchronize()
 
 
 # ----------------------------------------------------------------------------------------------------------------------------- tconv3

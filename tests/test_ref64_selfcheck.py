@@ -4,14 +4,20 @@ normalised slightly differently or one 64-key block missing).  The norm bounds r
 per-frame instead of joint-frame statistics and the fused-shift rounding on a constant row; the softmax bound a scale one fp16 ulp off;
 the mask and heat-map checks a resize index off by one (and the integer nearest index) and a white all-zero column; the step bound CFG
 guidance applied to the wrong half.  The GroupNorm statistics-exchange check rejects sets read as [F_loc, B], the own rank counted twice,
-non-first slots left unzeroed and a rounding to fp32 after every rank's add (or of the set total).  No GPU: everything here is fp64 on the CPU."""
+non-first slots left unzeroed and a rounding to fp32 after every rank's add (or of the set total).  The VAE block check (check_block on
+the fp16 floor, with the fp16 run emulated by a rounding to fp16 after every op) rejects q and k swapped, a softmax scale of 1/C or C^-1/4,
+a softmax over the queries, the value bias dropped or carried through the un-normalised probabilities, quant_conv folded with its weight
+transposed, the padded conv_out read one column late, downsample padding on the left / top, GroupNorm eps 1e-5 on a near-constant group
+and the nearest-upsample index off by one.  No GPU: everything here is fp64 on the CPU."""
 import pytest
 import torch
 import torch.nn.functional as F
 
-from _ref64 import (X_A, X_ALPHA, X_EQ, X_M, X_MAP, blend_mask_ratio, cfg_ddim_ref, check_attn, check_edit, check_heatmaps, check_mask,
-                    check_gn_combine, check_probs, check_running_sum, check_step, check_tap, cross_edit_ref, cross_edit_table, ddim_invert_ref,
-                    gemm_ref, gn_check, heatmap_values, ln_check, nearest_index, softmax64, ulp16)
+from _ref64 import (X_A, X_ALPHA, X_EQ, X_M, X_MAP, VaeBlocks64, blend_mask_ratio, cfg_ddim_ref, check_attn, check_block, check_edit,
+                    check_heatmaps, check_mask, check_gn_combine, check_probs, check_running_sum, check_step, check_tap, conv3x3_ref,
+                    conv3x3_rows_ref, cross_edit_ref, cross_edit_table, ddim_invert_ref, gemm_ref, gn_check, heatmap_values, ln_check,
+                    nearest_index, softmax64, ulp16, vae_block_state_dict)
+from oracle.vae_oracle import vae_param_spec
 
 
 def rnd(*shape, seed=0, scale=1.0):
@@ -410,3 +416,70 @@ def test_gn_combine_rejects(bug):
         got = fold64(rank_sum(own, peers, me), F_loc).float().double()
     with pytest.raises(AssertionError, match="are not 0" if bug == "rest_not_zeroed" else "differ from the fp64 replay"):
         check_gn_combine(got, own, peers, me, F_loc)
+
+
+# ------------------------------------------------------------------------------------------------------------------------ VAE blocks
+@pytest.mark.parametrize("stride,asym", [(1, False), (2, False), (2, True)])
+def test_conv_rows_ref_matches_full_conv(stride, asym):
+    """The row-gathered conv reference of the sampled VAE checks equals the full fp64 conv on the rows it is asked for."""
+    x, w9 = rnd(2, 6, 10, 16, seed=110).half(), rnd(9, 5, 16, seed=111, scale=0.1).half()
+    bias, res = rnd(5, seed=112), rnd(2 * (6 // stride) * (10 // stride), 5, seed=113).half()
+    ref, terms = conv3x3_ref(x, w9, stride, asym, bias=bias, residuals=(res,))
+    rows = torch.tensor([0, 3, 7, ref.shape[0] - 1, ref.shape[0] // 2])
+    r2, t2 = conv3x3_rows_ref(x, w9, rows, stride, asym, bias=bias, residuals=(res[rows],))
+    assert torch.allclose(r2, ref[rows], rtol=1e-13, atol=1e-13) and torch.allclose(t2, terms[rows], rtol=1e-13, atol=1e-13)
+
+
+VAE_SMALL = dict(in_channels=3, out_channels=3, block_out_channels=(32, 64), layers_per_block=1, latent_channels=4, norm_num_groups=8)
+to16 = lambda t: t.half().double()  # noqa: E731  (an fp16 run emulated in fp64: one rounding after every op)
+
+
+def vae_block_inputs():
+    """Small NCHW fp16 inputs of every block; the resnet input's first group (4 channels) is near-constant (sigma 1e-3: var ~ eps)."""
+    x = rnd(1, 32, 8, 8, seed=120).half()
+    x[:, :4] = (1e-3 * rnd(1, 4, 8, 8, seed=121)).half()
+    return dict(resnet_eps=("encoder.down_blocks.1.resnets.0", "resnet", rnd(1, 32, 8, 8, seed=122).half()),
+                resnet_const=("encoder.down_blocks.0.resnets.0", "resnet", x),
+                attn=("encoder.mid_block.attentions.0", "attn", rnd(1, 64, 8, 8, seed=123).half()),
+                down=("encoder.down_blocks.0.downsamplers.0", "down", rnd(1, 32, 8, 8, seed=124).half()),
+                up=("decoder.up_blocks.0.upsamplers.0", "up", rnd(1, 64, 4, 4, seed=125).half()),
+                encoder_in=(None, "encoder_in", (2 * torch.rand(1, 3, 8, 8, generator=torch.Generator().manual_seed(126)) - 1).half()),
+                encoder_out=(None, "encoder_out", rnd(1, 64, 4, 4, seed=127).half()),
+                decoder_in=(None, "decoder_in", (0.8 * rnd(1, 4, 4, 4, seed=128)).half()),
+                decoder_out=(None, "decoder_out", rnd(1, 32, 8, 8, seed=129).half()))
+
+
+def run_block(sd, block, rnd16=False, bug=None, probs=None):
+    name, method, x = vae_block_inputs()[block]
+    r = VaeBlocks64(sd, torch.float64, "cpu", groups=VAE_SMALL["norm_num_groups"], rnd=to16 if rnd16 else None, bug=bug)
+    args = (x.double(),) if name is None else (name, x.double())
+    return getattr(r, method)(*args, **({} if probs is None else dict(probs_out=probs)))
+
+
+@pytest.fixture(scope="module")
+def vae_sd():
+    return {k: v.double() for k, v in vae_block_state_dict(vae_param_spec(VAE_SMALL), seed=7).items()}
+
+
+def test_block_check_accepts_fp16_and_fp32(vae_sd):
+    for block in vae_block_inputs():
+        probs = [] if block == "attn" else None
+        ref = run_block(vae_sd, block, probs=probs)
+        o16 = run_block(vae_sd, block, rnd16=True)
+        check_block(o16, ref, o16)
+        check_block(ref.half(), ref, o16)
+        check_block(ref.float(), ref, o16)
+        if probs:  # the attention is peaked, so that what P selects matters
+            assert probs[0].amax(-1).median().item() > 0.5
+
+
+@pytest.mark.parametrize("block,bug", [("attn", "qk_swapped"), ("attn", "scale_1_over_c"), ("attn", "scale_c_quarter"),
+                                       ("attn", "softmax_over_queries"), ("attn", "vbias_dropped"), ("attn", "vbias_unnormalised"),
+                                       ("encoder_out", "quant_wq_transposed"), ("encoder_out", "conv_out_col_offset"),
+                                       ("decoder_out", "conv_out_col_offset"), ("down", "down_pad_left_top"),
+                                       ("resnet_const", "gn_eps_1e-5"), ("up", "upsample_index_off_by_one")])
+def test_block_check_rejects(vae_sd, block, bug):
+    ref = run_block(vae_sd, block)
+    o16 = run_block(vae_sd, block, rnd16=True)
+    with pytest.raises(AssertionError, match="fp16 floor"):
+        check_block(run_block(vae_sd, block, rnd16=True, bug=bug), ref, o16)
