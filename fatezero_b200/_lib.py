@@ -115,6 +115,7 @@ SIGNATURES = {
     "fz_softmax_rows_f16": [c_void_p, c_ll, c_int, c_ll, c_float, c_void_p],
     "fz_embed_tokens_f16": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     "fz_quick_gelu_f16": [c_void_p, c_ll, c_void_p],
+    "fz_gelu_f16": [c_void_p, c_ll, c_void_p],
     "fz_cross_heatmaps": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
     "fz_frames_to_u8": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p],
     "fz_resize_bicubic_u8": [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int,

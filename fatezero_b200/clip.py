@@ -1,7 +1,8 @@
 """CLIP text encoder on the sm_90a kernels (SURVEY.md §8(f) rank 4).  The reference encodes prompts with transformers' CLIPTextModel
 (`pipelines/stable_diffusion.py:230,279`: `self.text_encoder(ids, attention_mask=...)[0]`); `ClipTextEngine` executes the same pre-LN
-transformer (token + position embedding, 12 x {LN, causal self-attention, LN, quick_gelu MLP}, final LN) with fz_layernorm / fz_gemm /
-fz_attention (causal = 1) / fz_quick_gelu: fp16 storage, fp32 accumulation, fp32 output.  Weights are read from a CLIPTextModel-shaped
+transformer (token + position embedding, N x {LN, causal self-attention, LN, quick_gelu / gelu MLP}, final LN) with fz_layernorm / fz_gemm /
+fz_attention (causal = 1) / fz_quick_gelu (SD-1.x) or fz_gelu (the exact-erf GELU of the SD-2.x OpenCLIP text towers): fp16 storage,
+fp32 accumulation, fp32 output.  Weights are read from a CLIPTextModel-shaped
 state dict (`text_model.*` names); anything else (attention masks, projection heads, other activations) is refused, and the pipeline then
 keeps calling the caller's module."""
 from __future__ import annotations
@@ -15,11 +16,17 @@ from . import ops
 f16, f32 = torch.float16, torch.float32
 
 
+# transformers' CLIPMLP activation (config.hidden_act) -> the in-place kernel that computes it
+ACTIVATIONS = {"quick_gelu": ops.quick_gelu_, "gelu": ops.gelu_}
+
+
 class ClipTextEngine:
     def __init__(self, text_encoder: torch.nn.Module):
         cfg = text_encoder.config
-        if getattr(cfg, "hidden_act", "quick_gelu") != "quick_gelu":
-            raise NotImplementedError(f"CLIP hidden_act {cfg.hidden_act!r} (SD-1.x text encoders use quick_gelu)")
+        act = getattr(cfg, "hidden_act", "quick_gelu")
+        if act not in ACTIVATIONS:
+            raise NotImplementedError(f"CLIP hidden_act {act!r} (SD-1.x text encoders use quick_gelu, SD-2.x gelu)")
+        self.act = ACTIVATIONS[act]
         sd: Dict[str, torch.Tensor] = {k: v.detach() for k, v in text_encoder.state_dict().items()}
         dev = next(text_encoder.parameters()).device
         if dev.type != "cuda":
@@ -64,14 +71,15 @@ class ClipTextEngine:
             raise ValueError(f"{L} tokens > max_position_embeddings {self.L}")
         with torch.cuda.device(self.dev):
             x = ops.embed_tokens(self.tok, self.pos, input_ids.to(self.dev))
-            x = transformer_blocks(x, self.layers, B, L, self.C, self.heads, self.eps, causal=True)
+            x = transformer_blocks(x, self.layers, B, L, self.C, self.heads, self.eps, causal=True, act=self.act)
             out = ops.layernorm(x, *self.ln_f, eps=self.eps)
         return (out.float().view(B, L, self.C),)
 
 
-def transformer_blocks(x: torch.Tensor, layers, B: int, L: int, C: int, heads: int, eps: float, causal: bool) -> torch.Tensor:
+def transformer_blocks(x: torch.Tensor, layers, B: int, L: int, C: int, heads: int, eps: float, causal: bool,
+                       act=ops.quick_gelu_) -> torch.Tensor:
     """The pre-LN CLIP residual blocks on the current device: x [B*L, C] fp16 (B <= 64 sequences of L tokens, fz_attention_f16's row
-    limit) through {LN, self-attention, LN, quick_gelu MLP} per layer dict (ln1, ln2, qkv_w / qkv_b with q | k | v rows, out_w / out_b,
+    limit) through {LN, self-attention, LN, MLP with the in-place activation `act`} per layer dict (ln1, ln2, qkv_w / qkv_b with q | k | v rows, out_w / out_b,
     fc1_w / fc1_b, fc2_w / fc2_b)."""
     d = C // heads
     ld = (L + 7) // 8 * 8
@@ -84,6 +92,6 @@ def transformer_blocks(x: torch.Tensor, layers, B: int, L: int, C: int, heads: i
                       src_index=[list(range(B))], causal=causal)
         x = ops.gemm(o, ly["out_w"], bias=ly["out_b"], residual=x)
         hn = ops.layernorm(x, *ly["ln2"], eps=eps)
-        m = ops.quick_gelu_(ops.gemm(hn, ly["fc1_w"], bias=ly["fc1_b"]))
+        m = act(ops.gemm(hn, ly["fc1_w"], bias=ly["fc1_b"]))
         x = ops.gemm(m, ly["fc2_w"], bias=ly["fc2_b"], residual=x)
     return x

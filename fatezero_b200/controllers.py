@@ -840,22 +840,23 @@ def map_cache_bytes(unet_config: dict, model_config: dict, h: int, w: int, save_
     """HBM of one clip frame's inversion map cache at latent size h x w: (bytes per DDIM step, bytes held once: the cross running sums).
     Restates the slab shapes AttentionStore allocates for the UNet's transformer layers (self maps [heads, S, n_slots S], cross maps
     [heads, S, 80] and their sums, for S <= 32^2) so that a batch can be admitted before any of it is allocated."""
+    from .unet import level_heads
     ch = list(unet_config["block_out_channels"])
-    heads = int(unet_config["attention_head_dim"])
+    lh = level_heads(unet_config)  # SD-2.x stores 5 / 10 / 20 heads at the 64 / 32 / 16-pixel levels of a 512^2 clip, SD-1.x 8 everywhere
     lpb = int(unet_config["layers_per_block"])
     nblk = len(ch)
-    layers = []  # (channels, S)
+    layers = []  # (channels, heads, S)
     for i, t in enumerate(unet_config["down_block_types"]):
         if t.startswith("CrossAttn"):
-            layers += [(ch[i], (h >> i) * (w >> i))] * lpb
-    layers.append((ch[-1], (h >> (nblk - 1)) * (w >> (nblk - 1))))
+            layers += [(ch[i], lh[i], (h >> i) * (w >> i))] * lpb
+    layers.append((ch[-1], lh[-1], (h >> (nblk - 1)) * (w >> (nblk - 1))))
     for i, t in enumerate(unet_config["up_block_types"]):
         if t.startswith("CrossAttn"):
             s = nblk - 1 - i
-            layers += [(ch[s], (h >> s) * (w >> s))] * (lpb + 1)
+            layers += [(ch[s], lh[s], (h >> s) * (w >> s))] * (lpb + 1)
     index_list = list(model_config.get("SparseCausalAttention_index", [-1, "first"]))
     per_step = once = 0
-    for c, S in layers:
+    for c, heads, S in layers:
         if S > 32 ** 2:
             continue
         slots = len(index_list) if index_list and not ("least_sc_channel" in model_config and c < model_config["least_sc_channel"]) else 1

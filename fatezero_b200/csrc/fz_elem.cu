@@ -1146,6 +1146,13 @@ __global__ void quick_gelu_kernel(__half* __restrict__ x, long long n) {
     x[i] = __float2half_rn(v / (1.0f + __expf(-1.702f * v)));
   }
 }
+// exact (erf) GELU of the SD-2 text encoders' MLP: 0.5 v (1 + erf(v / sqrt 2)), as torch.nn.functional.gelu(approximate="none")
+__global__ void gelu_kernel(__half* __restrict__ x, long long n) {
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float v = __half2float(x[i]);
+    x[i] = __float2half_rn(0.5f * v * (1.0f + erff(v * 0.70710678118654752f)));
+  }
+}
 }  // namespace fz
 
 extern "C" int fz_embed_tokens_f16(const float* tok, const float* pos, const long long* ids, void* out, int rows, int L, int C, cudaStream_t stream) {
@@ -1157,6 +1164,12 @@ extern "C" int fz_embed_tokens_f16(const float* tok, const float* pos, const lon
 extern "C" int fz_quick_gelu_f16(void* x, long long n, cudaStream_t stream) {
   FZ_CHECK_ARG(x && n > 0, "fz_quick_gelu: bad args");
   fz::quick_gelu_kernel<<<static_cast<int>(std::min<long long>((n + 255) / 256, 132 * 8)), 256, 0, stream>>>(static_cast<__half*>(x), n);
+  FZ_CUDA(cudaGetLastError());
+  return FZ_OK;
+}
+extern "C" int fz_gelu_f16(void* x, long long n, cudaStream_t stream) {
+  FZ_CHECK_ARG(x && n > 0, "fz_gelu: bad args");
+  fz::gelu_kernel<<<static_cast<int>(std::min<long long>((n + 255) / 256, 132 * 8)), 256, 0, stream>>>(static_cast<__half*>(x), n);
   FZ_CUDA(cudaGetLastError());
   return FZ_OK;
 }

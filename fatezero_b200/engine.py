@@ -19,6 +19,7 @@ import torch
 import ctypes as C
 
 from . import _lib, ops
+from .unet import transformer_heads
 
 f16 = torch.float16
 f32 = torch.float32
@@ -58,7 +59,7 @@ class UNetEngine:
         self.cfg = dict(unet.config)
         self.mc = dict(unet.model_config)
         self.dev = dev
-        self.heads = self.cfg["attention_head_dim"]
+        self.heads = transformer_heads(self.cfg)  # transformer prefix -> head count of its level (SD-2.x: 5 / 10 / 20 / 20)
         self.groups = self.cfg["norm_num_groups"]
         self.eps = float(self.cfg["norm_eps"])
         self.ch = list(self.cfg["block_out_channels"])
@@ -307,10 +308,13 @@ class UNetEngine:
         for name in self.w:
             if name.endswith("attn2.kv"):
                 wkv = self.w[name]
+                if wkv.shape[1] != D:
+                    raise ValueError(f"encoder_hidden_states width {D} != cross_attention_dim {wkv.shape[1]}")
+                heads = self.heads[name[: -len(".transformer_blocks.0.attn2.kv")]]
                 c = wkv.shape[0] // 2
-                d = c // self.heads
-                vt = torch.zeros((B, self.heads, d, 80), dtype=f16, device=self.dev)
-                k = ops.gemm(t16, wkv, vt=dict(out=vt, col_start=c, S=L, d=d, heads=self.heads, ld=80))
+                d = c // heads
+                vt = torch.zeros((B, heads, d, 80), dtype=f16, device=self.dev)
+                k = ops.gemm(t16, wkv, vt=dict(out=vt, col_start=c, S=L, d=d, heads=heads, ld=80))
                 self._text_kv[name[: -len(".kv")]] = (k, vt)
         self._text_key = key
         self._text_ref = text  # keep alive so data_ptr stays unique
@@ -372,7 +376,7 @@ class UNetEngine:
         NB, H, W, C = x.shape
         S = H * W
         M = NB * S
-        heads = self.heads
+        heads = self.heads[p]
         d = C // heads
         scale = d ** -0.5
         bp = p + ".transformer_blocks.0"

@@ -290,10 +290,20 @@ def cfg_ddim_step_multi(x: torch.Tensor, eps2: torch.Tensor, guidance: float, a_
               _stream())
 
 
+def _same_map_geometry(maps: Sequence[torch.Tensor], what: str):
+    """The map kernels read every map with the first one's [F, heads, r*r] and row stride and average over maps x heads: a map of another
+    head count (SD-2.x stores 5 / 10 / 20 heads at different levels) would be misread and misweighted."""
+    m0 = maps[0]
+    for m in maps[1:]:
+        if m.shape[:3] != m0.shape[:3] or m.stride(2) != m0.stride(2) or m.dtype != m0.dtype:
+            raise ValueError(f"fatezero_b200.ops.{what}: maps of different geometry {tuple(m.shape)} vs {tuple(m0.shape)} in one call")
+
+
 def blend_mask(maps: Sequence[torch.Tensor], word_w: torch.Tensor, th: float, h: int, w: int) -> torch.Tensor:
     """maps: list of [F, heads, r*r, ld] (fp16 cache slabs or fp16 running sums) -> mask [F, h, w] float 0/1."""
     m0 = maps[0]
     Fm, heads, rr, ld = m0.shape
+    _same_map_geometry(maps, "blend_mask")
     r = int(round(rr ** 0.5))
     arr = (C.c_void_p * len(maps))(*[m.data_ptr() for m in maps])
     ww = [float(v) for v in word_w.tolist()]
@@ -325,6 +335,14 @@ def quick_gelu_(x: torch.Tensor) -> torch.Tensor:
     _chk(x, f16, "quick_gelu")
     assert x.is_contiguous()
     _lib.call("fz_quick_gelu_f16", _p(x), x.numel(), _stream())
+    return x
+
+
+def gelu_(x: torch.Tensor) -> torch.Tensor:
+    """Exact (erf) GELU in place: the MLP activation of SD-2 text encoders (hidden_act "gelu")."""
+    _chk(x, f16, "gelu")
+    assert x.is_contiguous()
+    _lib.call("fz_gelu_f16", _p(x), x.numel(), _stream())
     return x
 
 
@@ -410,6 +428,7 @@ def cross_heatmaps(maps: Sequence[torch.Tensor], ntok: int) -> torch.Tensor:
     """maps: cross-attention running sums [F, heads, r*r, ld] (fp16 or fp32) of ONE resolution -> uint8 [F, ntok, r, r] heat maps."""
     m0 = maps[0]
     Fm, heads, rr, _ = m0.shape
+    _same_map_geometry(maps, "cross_heatmaps")
     r = int(round(rr ** 0.5))
     arr = (C.c_void_p * len(maps))(*[m.data_ptr() for m in maps])
     out = torch.empty((Fm, ntok, r, r), dtype=torch.uint8, device=m0.device)

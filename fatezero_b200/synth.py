@@ -30,7 +30,16 @@ MINI_UNET_CONFIG = dict(SD14_UNET_CONFIG, block_out_channels=(64, 128, 256, 256)
 MID_UNET_CONFIG = dict(SD14_UNET_CONFIG, block_out_channels=(160, 320, 640, 640), attention_head_dim=4,
                        cross_attention_dim=256)
 
-UNET_CONFIGS = {"sd14": SD14_UNET_CONFIG, "mini": MINI_UNET_CONFIG, "mid": MID_UNET_CONFIG}
+# SD-2.0 / 2.1-base `unet/config.json` values: heads per block 5 / 10 / 20 / 20 (head dim 64 at every level), linear proj_in / proj_out,
+# 1024-wide OpenCLIP text (the text stand-in is ToyTextEncoder(1024)).
+SD2_UNET_CONFIG = dict(SD14_UNET_CONFIG, attention_head_dim=(5, 10, 20, 20), cross_attention_dim=1024, use_linear_projection=True,
+                       upcast_attention=False)
+
+# Small SD-2 geometry: same topology and head dim 64 at every level (heads 1 / 2 / 4 / 4), 1024-wide text.
+SD2_MINI_UNET_CONFIG = dict(SD2_UNET_CONFIG, block_out_channels=(64, 128, 256, 256), attention_head_dim=(1, 2, 4, 4))
+
+UNET_CONFIGS = {"sd14": SD14_UNET_CONFIG, "mini": MINI_UNET_CONFIG, "mid": MID_UNET_CONFIG, "sd2": SD2_UNET_CONFIG,
+                "sd2mini": SD2_MINI_UNET_CONFIG}
 
 DEFAULT_MODEL_CONFIG = dict(lora=160, SparseCausalAttention_index=["mid"], least_sc_channel=640)
 

@@ -3,7 +3,8 @@
 
 The module owns fp32 parameters under EXACTLY the reference's state-dict names / shapes (SURVEY.md App. E3), so
 `from_2d_model` / `load_2d_state_dict` / `load_state_dict` accept Stable-Diffusion-1.x and Tune-A-Video checkpoints
-unchanged.  `forward` does not run PyTorch layers: it hands the tensors to `engine.UNetEngine`, which executes the
+unchanged, and so do Stable-Diffusion-2.x base configurations (per-block `attention_head_dim`, `use_linear_projection`,
+`upcast_attention`, 1024-wide text).  `forward` does not run PyTorch layers: it hands the tensors to `engine.UNetEngine`, which executes the
 step with the sm_90a kernels of libfatezero_b200.so (there is no CPU / eager fallback).
 """
 from __future__ import annotations
@@ -13,7 +14,7 @@ import json
 import math
 import os
 from collections import OrderedDict
-from typing import Dict, Optional, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 from torch import nn
@@ -40,14 +41,45 @@ def lora_rank(requested: int, channels: int) -> int:
     return requested if requested <= channels else channels // 2
 
 
+def level_heads(cfg: dict) -> List[int]:
+    """Attention heads of the transformers at each resolution level.  `attention_head_dim` is the head COUNT per block (diffusers 0.11.1
+    semantics, unet_3d_condition.py:115-116,164,195,217 -> unet_3d_blocks.py:177-179): one int for every block (SD-1.x: 8) or one entry
+    per down block (SD-2.x: 5 / 10 / 20 / 20, head dim 64).  Down block i uses entry i, the mid block the last entry and up block i the
+    reversed list's entry i, so every block at level l runs entry l."""
+    ch = list(cfg["block_out_channels"])
+    hd = cfg["attention_head_dim"]
+    heads = [int(hd)] * len(ch) if isinstance(hd, int) else [int(h) for h in hd]
+    if len(heads) != len(ch) or any(h < 1 or c % h for h, c in zip(heads, ch)):
+        raise ValueError(f"attention_head_dim {hd!r} does not give a head count dividing each of block_out_channels {tuple(ch)}")
+    return heads
+
+
+def transformer_heads(cfg: dict) -> "OrderedDict[str, int]":
+    """State-dict prefix of every transformer of the UNet (forward order) -> its head count (level_heads)."""
+    heads = level_heads(cfg)
+    nblk = len(heads)
+    lpb = int(cfg["layers_per_block"])
+    out: "OrderedDict[str, int]" = OrderedDict()
+    for i, t in enumerate(cfg["down_block_types"]):
+        if t.startswith("CrossAttn"):
+            for j in range(lpb):
+                out[f"down_blocks.{i}.attentions.{j}"] = heads[i]
+    out["mid_block.attentions.0"] = heads[-1]
+    for i, t in enumerate(cfg["up_block_types"]):
+        if t.startswith("CrossAttn"):
+            for j in range(lpb + 1):
+                out[f"up_blocks.{i}.attentions.{j}"] = heads[nblk - 1 - i]
+    return out
+
+
 def unet_param_spec(cfg: dict, model_config: dict) -> "OrderedDict[str, Tuple[tuple, str]]":
     """name -> (shape, init kind) for every tensor of the reference state dict (902 tensors for SD-1.4 + lora:160)."""
     spec: "OrderedDict[str, Tuple[tuple, str]]" = OrderedDict()
     ch = list(cfg["block_out_channels"])
     c0 = ch[0]
     temb = 4 * c0
-    heads = cfg["attention_head_dim"]
     dtext = cfg["cross_attention_dim"]
+    linear_proj = bool(cfg.get("use_linear_projection", False))
     lpb = cfg["layers_per_block"]
     mc = model_config or {}
 
@@ -83,7 +115,11 @@ def unet_param_spec(cfg: dict, model_config: dict) -> "OrderedDict[str, Tuple[tu
 
     def transformer(name, c):
         norm(f"{name}.norm", c)
-        conv(f"{name}.proj_in", c, c, 1)
+        # use_linear_projection (SD-2.x): proj_in / proj_out are nn.Linear [C, C] instead of 1x1 convs (models/attention.py:63-66,90-93)
+        if linear_proj:
+            linear(f"{name}.proj_in", c, c)
+        else:
+            conv(f"{name}.proj_in", c, c, 1)
         b = f"{name}.transformer_blocks.0"
         for proj in ("to_q", "to_k", "to_v"):
             linear(f"{b}.attn1.{proj}", c, c, bias=False)
@@ -102,7 +138,10 @@ def unet_param_spec(cfg: dict, model_config: dict) -> "OrderedDict[str, Tuple[tu
         linear(f"{b}.ff.net.0.proj", c, 8 * c)
         linear(f"{b}.ff.net.2", 4 * c, c)
         norm(f"{b}.norm3", c)
-        conv(f"{name}.proj_out", c, c, 1)
+        if linear_proj:
+            linear(f"{name}.proj_out", c, c)
+        else:
+            conv(f"{name}.proj_out", c, c, 1)
 
     conv("conv_in", cfg["in_channels"], c0, 3)
     linear("time_embedding.linear_1", c0, temb)
@@ -186,6 +225,12 @@ _MODEL_CONFIG_KEYS = ("lora", "SparseCausalAttention_index", "least_sc_channel",
 
 
 class UNetPseudo3DConditionModel(nn.Module):
+    """Drop-in for the reference's UNetPseudo3DConditionModel (SD-1.x and SD-2.x base configurations).
+
+    `upcast_attention=True` is accepted and changes nothing: every attention kernel forms Q.K^T from fp16 operands with fp32
+    accumulation and runs the softmax in fp32, which is what upcasting asks of an fp16 model.  Only epsilon-prediction checkpoints are
+    meaningful (the reference's DDIM inversion assumes epsilon); v-prediction (SD-2.x 768-v) checkpoints load but are not converted."""
+
     def __init__(self, **kwargs):
         super().__init__()
         cfg = dict(_SD_DEFAULTS)
@@ -205,18 +250,17 @@ class UNetPseudo3DConditionModel(nn.Module):
     def _check_supported(cfg):
         def bad(msg):
             raise NotImplementedError(f"fatezero_b200 UNet: {msg} is not on the FateZero SD-1.x hot path")
-        if cfg["use_linear_projection"] or cfg["dual_cross_attention"]:
-            bad("use_linear_projection / dual_cross_attention")
+        if cfg["dual_cross_attention"]:
+            bad("dual_cross_attention")
         if cfg["class_embed_type"] is not None or cfg["num_class_embeds"] is not None:
             bad("class embeddings")
         if cfg["resnet_time_scale_shift"] != "default":
             bad("resnet_time_scale_shift != 'default'")
         if cfg.get("temporal_downsample") or cfg.get("temporal_downsample_time"):
             bad("temporal_downsample (commented out in every shipped YAML)")
-        if cfg["only_cross_attention"] not in (False, [False] * 4, (False,) * 4) or cfg["upcast_attention"]:
-            bad("only_cross_attention / upcast_attention")
-        if not isinstance(cfg["attention_head_dim"], int):
-            bad("per-block attention_head_dim")
+        if cfg["only_cross_attention"] not in (False, [False] * 4, (False,) * 4):
+            bad("only_cross_attention")
+        level_heads(cfg)
         if cfg["center_input_sample"]:
             bad("center_input_sample")
         if cfg["act_fn"] not in ("silu", "swish"):

@@ -212,6 +212,9 @@ int fz_blend_mask(const void* const* maps, int num_maps, int maps_f32, int F, in
  * out[r, :] = fp16(tok[ids[r], :] + pos[r % L, :]) and the quick_gelu activation x * sigmoid(1.702 x) in place. */
 int fz_embed_tokens_f16(const float* tok, const float* pos, const long long* ids, void* out, int rows, int L, int C, fz_stream_t stream);
 int fz_quick_gelu_f16(void* x, long long n, fz_stream_t stream);
+/* exact GELU 0.5 x (1 + erf(x / sqrt 2)) in place, fp32 math with erff: the MLP activation of the SD-2 text encoders (hidden_act "gelu",
+ * transformers' CLIPMLP.forward -> ACT2FN["gelu"] = torch.nn.functional.gelu without the tanh approximation) */
+int fz_gelu_f16(void* x, long long n, fz_stream_t stream);
 
 /* in-place row softmax x[r, :n] <- softmax(scale * x[r, :n]), fp32 math: the VAE's 512-wide single-head attention runs GEMM -> this -> GEMM */
 int fz_softmax_rows_f16(void* x, long long rows, int n, long long ld, float scale, fz_stream_t stream);
