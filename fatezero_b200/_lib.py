@@ -104,6 +104,8 @@ SIGNATURES = {
                                C.POINTER(c_void_p), C.POINTER(c_int), c_ll, c_void_p],
     "fz_blend_mask": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(c_float), c_float, c_int, c_int,
                       c_void_p, c_void_p],
+    "fz_blend_mask_hw": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(c_float), c_float, c_int,
+                         c_int, c_void_p, c_void_p],
     "fz_p2p_alloc": [c_ll, C.POINTER(c_void_p)],
     "fz_p2p_free": [c_void_p],
     "fz_p2p_export": [c_void_p, c_void_p],
@@ -117,6 +119,7 @@ SIGNATURES = {
     "fz_quick_gelu_f16": [c_void_p, c_ll, c_void_p],
     "fz_gelu_f16": [c_void_p, c_ll, c_void_p],
     "fz_cross_heatmaps": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "fz_cross_heatmaps_hw": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
     "fz_frames_to_u8": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p],
     "fz_resize_bicubic_u8": [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
                              c_void_p, c_void_p, c_void_p],

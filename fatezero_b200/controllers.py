@@ -22,7 +22,7 @@ from typing import Dict, List, Optional, Tuple, Union
 import torch
 
 from . import _lib, tables
-from .spatial_blend import SpatialBlender
+from .spatial_blend import SpatialBlender, level_hw
 
 KEYS = ("down_cross", "mid_cross", "up_cross", "down_self", "mid_self", "up_self")
 CROSS_LD = 80  # 77 text tokens padded so cache rows are 16-byte multiples (TMA store / vector access)
@@ -54,6 +54,7 @@ class AttentionControl(abc.ABC):
         self.cur_step = 0
         self.num_att_layers = -1
         self.cur_att_layer = 0
+        self._latent_hw: Optional[Tuple[int, int]] = None  # the clip's latent (h, w), given by the UNet engine at every forward
 
     def step_callback(self, x_t):
         self.cur_att_layer = 0
@@ -78,8 +79,11 @@ class AttentionControl(abc.ABC):
         self.cur_att_layer = 0
 
     # ---- fused-kernel protocol (called by engine.UNetEngine) ----------------------------------------------------
-    def begin_forward(self, batch: int, frames: int):
+    def begin_forward(self, batch: int, frames: int, latent_hw: Optional[Tuple[int, int]] = None):
+        """latent_hw: the (h, w) of the clip's latents: a stored map of S pixels is then the level_hw(S, h, w) grid (non-square clips)."""
         self._pos = {k: 0 for k in KEYS}
+        if latent_hw is not None:
+            self._latent_hw = (int(latent_hw[0]), int(latent_hw[1]))
 
     def _edit_start(self, nb: int) -> int:
         return 0 if self.LOW_RESOURCE else nb // 2
@@ -273,7 +277,7 @@ class AttentionStore(AttentionControl):
     # ---- CUDA-graph replay support (graphs.py): the launch sequence of a loop depends on the controller only through this signature;
     # after a replay the captured controller's end-of-loop state (same slabs, refilled) is adopted by the caller's controller object ----
     _ADOPT = ("cur_step", "cur_att_layer", "step_store", "_acc", "_self_sum_cache", "latents_store", "attention_store_all_step",
-              "attention_store_paths", "_pos")
+              "attention_store_paths", "_pos", "_latent_hw")
 
     def graph_signature(self):
         if type(self) is not AttentionStore or self.disk_store or self.host_spill:
@@ -430,8 +434,8 @@ class AttentionControlEdit(AttentionStore, abc.ABC):
         return d
 
     # ---- fused protocol -------------------------------------------------------------------------------------------------
-    def begin_forward(self, batch, frames):
-        super().begin_forward(batch, frames)
+    def begin_forward(self, batch, frames, latent_hw=None):
+        super().begin_forward(batch, frames, latent_hw)
         if self.LOW_RESOURCE or batch != 2:
             raise RuntimeError("the edit controller expects a classifier-free-guidance batch (uncond, cond); LOW_RESOURCE is the "
                                "inversion mode (attention_store.py:40-46)")
@@ -451,13 +455,15 @@ class AttentionControlEdit(AttentionStore, abc.ABC):
             base = base.to(torch.cuda.current_device(), f16)
         start = self._edit_start(nb)
         if self.attention_blend is not None:
-            r = int(round(S ** 0.5))
-            ck = (step_in_store, r)
+            if self._latent_hw is None:
+                raise RuntimeError("the self-attention blend needs the clip's latent size: begin_forward(batch, frames, latent_hw)")
+            rh, rw = level_hw(S, *self._latent_hw)
+            ck = (step_in_store, (rh, rw))
             if ck not in self._mask_cache:
                 # prompt_choose == 'source': only the stored source maps enter, so the mask is shared by all layers of a step at
                 # one resolution (the reference recomputes it per layer: SURVEY.md K18)
                 self._mask_cache = {k: v for k, v in self._mask_cache.items() if k[0] == step_in_store}
-                m = self.attention_blend.mask_from(self._source_maps(step_in_store), 0, r, r)
+                m = self.attention_blend.mask_from(self._source_maps(step_in_store), 0, rh, rw, latent_hw=self._latent_hw)
                 self._mask_cache[ck] = m.reshape(m.shape[0], S).contiguous()
             self.attention_blend.counter += 1
             return dict(edit_bf_start=start, row_mode=_lib.ATTN_BLEND, base=base, cache_ld=T, mask=self._mask_cache[ck])
@@ -495,8 +501,8 @@ class AttentionControlEdit(AttentionStore, abc.ABC):
         lb = self.latent_blend
         src = self._source_maps(step_in_store)
         tgt = self.attention_store  # running sums including this step's pre-edit maps (updated in-kernel)
-        m_src = lb.mask_from(src, 0, h, w)
-        m_tgt = lb.mask_from(tgt, 1, h, w)
+        m_src = lb.mask_from(src, 0, h, w, latent_hw=(h, w))
+        m_tgt = lb.mask_from(tgt, 1, h, w, latent_hw=(h, w))
         lb.mask_list.append(m_src[:, None, :, :].float())
         lb.counter += 1
         apply = lb.start_blend < lb.counter < lb.end_blend
@@ -615,12 +621,15 @@ class AttentionControlEditBatch:
                 e.num_att_layers = value
 
     # ---- fused-kernel protocol ------------------------------------------------------------------------------------------
-    def begin_forward(self, batch, frames):
+    def begin_forward(self, batch, frames, latent_hw=None):
         if batch != 2 * self.prompt_groups:
             raise RuntimeError(f"AttentionControlEditBatch: expected a CFG batch of 2 x {self.prompt_groups} prompts, got {batch}")
         self._frames = frames
         for e in self.edits:
-            e.begin_forward(2, frames)
+            if latent_hw is None:  # a child with the two-argument protocol is asked exactly what it was asked before
+                e.begin_forward(2, frames)
+            else:
+                e.begin_forward(2, frames, latent_hw)
 
     def _merge(self, answers: List[Optional[dict]], frames: int) -> Optional[dict]:
         if self.prompt_groups == 1:
@@ -717,11 +726,11 @@ class AttentionStoreBatch:
         return self.stores[0].cur_step
 
     # ---- fused-kernel protocol ------------------------------------------------------------------------------------------
-    def begin_forward(self, batch, frames):
+    def begin_forward(self, batch, frames, latent_hw=None):
         if batch != self.prompt_groups:
             raise RuntimeError(f"AttentionStoreBatch: expected a batch of {self.prompt_groups} clips, got {batch}")
         for s in self.stores:
-            s.begin_forward(1, frames)
+            s.begin_forward(1, frames, latent_hw)
 
     def _merge(self, answers: List[Optional[dict]]) -> Optional[dict]:
         if self.prompt_groups == 1:

@@ -701,15 +701,16 @@ __global__ void cfg_ddim_kernel(float* __restrict__ x, const float* __restrict__
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Blend mask (spatial_blend.py:24-39, 78-111): mean over (layers, heads) of sum_n map[f,hd,p,n]*w[n] on the r x r grid,
+// Blend mask (spatial_blend.py:24-39, 78-111): mean over (layers, heads) of sum_n map[f,hd,p,n]*w[n] on the rh x rw grid,
 // 3x3 max-pool (stride 1, pad 1), nearest resize to (h, w), divide by the per-frame max, compare with th.
-// maps: up to 8 pointers to [F, heads, r*r, ldm] fp16 (or fp32 running sums when maps_f32 != 0). One CTA per frame.
+// maps: up to 8 pointers to [F, heads, rh*rw, ldm] fp16 (or fp32 running sums when maps_f32 != 0). One CTA per frame: the stored map
+// levels hold at most 32^2 pixels, so both grids fit the CTA's shared memory.
 // ---------------------------------------------------------------------------------------------------------------
 struct MaskParams {
   const void* maps[8];
   int num_maps;
   int maps_f32;
-  int F, heads, r, ldm, ntok;
+  int F, heads, rh, rw, ldm, ntok;
   float w[80];
   float th;
   int h, w_out;
@@ -718,11 +719,11 @@ struct MaskParams {
 
 __global__ void __launch_bounds__(256) blend_mask_kernel(const __grid_constant__ MaskParams p) {
   extern __shared__ float mk_smem[];
-  float* agg = mk_smem;              // [r*r]
-  float* pooled = mk_smem + p.r * p.r;  // [r*r]
+  const int rr = p.rh * p.rw;
+  float* agg = mk_smem;        // [rh*rw]
+  float* pooled = mk_smem + rr;  // [rh*rw]
   __shared__ float s_max;
   const int f = blockIdx.x;
-  const int rr = p.r * p.r;
   for (int px = threadIdx.x; px < rr; px += blockDim.x) {
     float a = 0.f;
     for (int l = 0; l < p.num_maps; ++l)
@@ -743,33 +744,33 @@ __global__ void __launch_bounds__(256) blend_mask_kernel(const __grid_constant__
   if (threadIdx.x == 0) s_max = 0.f;
   __syncthreads();
   for (int px = threadIdx.x; px < rr; px += blockDim.x) {
-    const int y = px / p.r, x = px % p.r;
+    const int y = px / p.rw, x = px % p.rw;
     float m = -INFINITY;
     for (int dy = -1; dy <= 1; ++dy)
       for (int dx = -1; dx <= 1; ++dx) {
         const int yy = y + dy, xx = x + dx;
-        if (yy >= 0 && yy < p.r && xx >= 0 && xx < p.r) m = fmaxf(m, agg[yy * p.r + xx]);
+        if (yy >= 0 && yy < p.rh && xx >= 0 && xx < p.rw) m = fmaxf(m, agg[yy * p.rw + xx]);
       }
     pooled[px] = m;
   }
   __syncthreads();
-  // F.interpolate(mode="nearest") source index: min(floor(dst * (float)in / out), in - 1) in fp32 (the exact integer quotient
+  // F.interpolate(mode="nearest") source index, per axis: min(floor(dst * (float)in / out), in - 1) in fp32 (the exact integer quotient
   // (dst * in) / out differs for some sizes, e.g. in = 16, out = 82)
-  const float sy_scale = static_cast<float>(p.r) / p.h, sx_scale = static_cast<float>(p.r) / p.w_out;
+  const float sy_scale = static_cast<float>(p.rh) / p.h, sx_scale = static_cast<float>(p.rw) / p.w_out;
   // max over the RESIZED grid == max over the source pixels that the nearest resize actually samples
   float lm = 0.f;
   for (int i = threadIdx.x; i < p.h * p.w_out; i += blockDim.x) {
     const int y = i / p.w_out, x = i % p.w_out;
-    const int sy = min(p.r - 1, static_cast<int>(floorf(y * sy_scale))), sx = min(p.r - 1, static_cast<int>(floorf(x * sx_scale)));
-    lm = fmaxf(lm, pooled[sy * p.r + sx]);
+    const int sy = min(p.rh - 1, static_cast<int>(floorf(y * sy_scale))), sx = min(p.rw - 1, static_cast<int>(floorf(x * sx_scale)));
+    lm = fmaxf(lm, pooled[sy * p.rw + sx]);
   }
   atomicMax(reinterpret_cast<int*>(&s_max), __float_as_int(fmaxf(lm, 0.f)));
   __syncthreads();
   const float mx = s_max;
   for (int i = threadIdx.x; i < p.h * p.w_out; i += blockDim.x) {
     const int y = i / p.w_out, x = i % p.w_out;
-    const int sy = min(p.r - 1, static_cast<int>(floorf(y * sy_scale))), sx = min(p.r - 1, static_cast<int>(floorf(x * sx_scale)));
-    const float v = pooled[sy * p.r + sx];
+    const int sy = min(p.rh - 1, static_cast<int>(floorf(y * sy_scale))), sx = min(p.rw - 1, static_cast<int>(floorf(x * sx_scale)));
+    const float v = pooled[sy * p.rw + sx];
     // reference: (v / mx) > th, with 0/0 = NaN -> False
     p.out[(static_cast<long long>(f) * p.h + y) * p.w_out + x] = (mx > 0.f && (v / mx) > p.th) ? 1.f : 0.f;
   }
@@ -1060,18 +1061,24 @@ extern "C" int fz_cfg_ddim_step_multi(float* x, const float* eps2, int K, long l
   return cfg_ddim_launch(x, eps2, K, n_item, guidance, a_t, a_prev, items, fhw, stream);
 }
 
-extern "C" int fz_blend_mask(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int r, int ldm, int ntok, const float* word_w,
-                             float th, int h, int w, float* out, cudaStream_t stream) {
-  FZ_CHECK_ARG(maps && word_w && out && num_maps >= 1 && num_maps <= 8 && ntok <= 80, "fz_blend_mask: bad args");
+extern "C" int fz_blend_mask_hw(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int rh, int rw, int ldm, int ntok,
+                                const float* word_w, float th, int h, int w, float* out, cudaStream_t stream) {
+  FZ_CHECK_ARG(maps && word_w && out && num_maps >= 1 && num_maps <= 8 && ntok <= 80 && rh >= 1 && rw >= 1 && rh * rw <= 1024,
+               "fz_blend_mask: bad args");
   MaskParams p;
   for (int i = 0; i < 8; ++i) p.maps[i] = i < num_maps ? maps[i] : nullptr;
-  p.num_maps = num_maps; p.maps_f32 = maps_f32; p.F = F; p.heads = heads; p.r = r; p.ldm = ldm; p.ntok = ntok;
+  p.num_maps = num_maps; p.maps_f32 = maps_f32; p.F = F; p.heads = heads; p.rh = rh; p.rw = rw; p.ldm = ldm; p.ntok = ntok;
   for (int i = 0; i < 80; ++i) p.w[i] = i < ntok ? word_w[i] : 0.f;  // word_w is a HOST array (77 floats, built once per edit)
   p.th = th; p.h = h; p.w_out = w; p.out = out;
-  const size_t smem = static_cast<size_t>(2 * r * r) * sizeof(float);
+  const size_t smem = static_cast<size_t>(2 * rh * rw) * sizeof(float);
   blend_mask_kernel<<<F, 256, smem, stream>>>(p);
   FZ_CUDA(cudaGetLastError());
   return FZ_OK;
+}
+
+extern "C" int fz_blend_mask(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int r, int ldm, int ntok, const float* word_w,
+                             float th, int h, int w, float* out, cudaStream_t stream) {
+  return fz_blend_mask_hw(maps, num_maps, maps_f32, F, heads, r, r, ldm, ntok, word_w, th, h, w, out, stream);
 }
 
 
@@ -1080,7 +1087,7 @@ namespace fz {
 // show_cross_attention on the device (prompt_attention/visualization.py:14-72): the heat map of text token `tok` in frame f is the mean
 // over the selected cross-attention maps (layers) and heads of the time-averaged probabilities, scaled to 0..255 by its own maximum.
 // The reference averages EVERY stored map (get_average_attention: self maps included) and moves the r16 cross maps to the host; here
-// one CTA per (frame, token) reads the running-sum slabs in place and emits res*res bytes — the means' constant factors cancel in v / max.
+// one CTA per (frame, token) reads the running-sum slabs in place and emits rh*rw bytes — the means' constant factors cancel in v / max.
 // ---------------------------------------------------------------------------------------------------------------
 struct HeatParams {
   const void* maps[8];
@@ -1117,15 +1124,21 @@ __global__ void __launch_bounds__(256) cross_heatmap_kernel(const __grid_constan
 
 }  // namespace fz
 
-extern "C" int fz_cross_heatmaps(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int res, int ldm, int ntok, unsigned char* out,
-                                 cudaStream_t stream) {
-  FZ_CHECK_ARG(maps && out && num_maps >= 1 && num_maps <= 8 && res * res <= 1024 && ntok >= 1 && ntok <= ldm, "fz_cross_heatmaps: bad args");
+extern "C" int fz_cross_heatmaps_hw(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int rh, int rw, int ldm, int ntok,
+                                    unsigned char* out, cudaStream_t stream) {
+  FZ_CHECK_ARG(maps && out && num_maps >= 1 && num_maps <= 8 && rh >= 1 && rw >= 1 && rh * rw <= 1024 && ntok >= 1 && ntok <= ldm,
+               "fz_cross_heatmaps: bad args");
   fz::HeatParams p;
   for (int i = 0; i < 8; ++i) p.maps[i] = i < num_maps ? maps[i] : nullptr;
-  p.num_maps = num_maps; p.maps_f32 = maps_f32; p.heads = heads; p.rr = res * res; p.ldm = ldm; p.ntok = ntok; p.out = out;
+  p.num_maps = num_maps; p.maps_f32 = maps_f32; p.heads = heads; p.rr = rh * rw; p.ldm = ldm; p.ntok = ntok; p.out = out;
   fz::cross_heatmap_kernel<<<dim3(ntok, F), 256, 0, stream>>>(p);
   FZ_CUDA(cudaGetLastError());
   return FZ_OK;
+}
+
+extern "C" int fz_cross_heatmaps(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int res, int ldm, int ntok, unsigned char* out,
+                                 cudaStream_t stream) {
+  return fz_cross_heatmaps_hw(maps, num_maps, maps_f32, F, heads, res, res, ldm, ntok, out, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

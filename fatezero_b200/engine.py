@@ -499,7 +499,7 @@ class UNetEngine:
             raise ValueError(f"batch {B} does not split into {groups} prompt groups")
         self._images_per_item = NB // groups if groups > 1 else None
         if ctrl is not None:
-            ctrl.begin_forward(B, F)
+            ctrl.begin_forward(B, F, (H, W))
         temb_all = self.time_embedding(t)
         xf = x.to(f32).contiguous()
         cols = ops.im2col_latents(xf)

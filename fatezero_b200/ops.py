@@ -3,7 +3,7 @@ streams, and nothing else — every compute call below lands in libfatezero_b200
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 import torch
 
@@ -299,17 +299,29 @@ def _same_map_geometry(maps: Sequence[torch.Tensor], what: str):
             raise ValueError(f"fatezero_b200.ops.{what}: maps of different geometry {tuple(m.shape)} vs {tuple(m0.shape)} in one call")
 
 
-def blend_mask(maps: Sequence[torch.Tensor], word_w: torch.Tensor, th: float, h: int, w: int) -> torch.Tensor:
-    """maps: list of [F, heads, r*r, ld] (fp16 cache slabs or fp16 running sums) -> mask [F, h, w] float 0/1."""
+def _map_grid(rr: int, hw, what: str) -> Tuple[int, int]:
+    """(rh, rw) of maps with rr pixels: `hw` when given, else the square grid (the reference's assumption)."""
+    if hw is None:
+        r = int(round(rr ** 0.5))
+        return r, r
+    rh, rw = int(hw[0]), int(hw[1])
+    if rh * rw != rr:
+        raise ValueError(f"fatezero_b200.ops.{what}: maps of {rr} pixels are not a {rh} x {rw} grid")
+    return rh, rw
+
+
+def blend_mask(maps: Sequence[torch.Tensor], word_w: torch.Tensor, th: float, h: int, w: int, hw=None) -> torch.Tensor:
+    """maps: list of [F, heads, rh*rw, ld] (fp16 cache slabs or fp16 running sums) -> mask [F, h, w] float 0/1.
+    hw = (rh, rw): the maps' grid; without it the grid is square."""
     m0 = maps[0]
     Fm, heads, rr, ld = m0.shape
     _same_map_geometry(maps, "blend_mask")
-    r = int(round(rr ** 0.5))
+    rh, rw = _map_grid(rr, hw, "blend_mask")
     arr = (C.c_void_p * len(maps))(*[m.data_ptr() for m in maps])
     ww = [float(v) for v in word_w.tolist()]
     wv = (C.c_float * len(ww))(*ww)
     out = torch.empty((Fm, h, w), dtype=torch.float32, device=m0.device)
-    _lib.call("fz_blend_mask", arr, len(maps), int(m0.dtype == torch.float32), Fm, heads, r, m0.stride(2), min(len(ww), 77), wv,
+    _lib.call("fz_blend_mask_hw", arr, len(maps), int(m0.dtype == torch.float32), Fm, heads, rh, rw, m0.stride(2), min(len(ww), 77), wv,
               float(th), h, w, _p(out), _stream())
     return out
 
@@ -424,15 +436,17 @@ def clip_scores(img: torch.Tensor, txt: torch.Tensor, clip_frames: Sequence[int]
     return o
 
 
-def cross_heatmaps(maps: Sequence[torch.Tensor], ntok: int) -> torch.Tensor:
-    """maps: cross-attention running sums [F, heads, r*r, ld] (fp16 or fp32) of ONE resolution -> uint8 [F, ntok, r, r] heat maps."""
+def cross_heatmaps(maps: Sequence[torch.Tensor], ntok: int, hw=None) -> torch.Tensor:
+    """maps: cross-attention running sums [F, heads, rh*rw, ld] (fp16 or fp32) of ONE resolution -> uint8 [F, ntok, rh, rw] heat maps.
+    hw = (rh, rw): the maps' grid; without it the grid is square."""
     m0 = maps[0]
     Fm, heads, rr, _ = m0.shape
     _same_map_geometry(maps, "cross_heatmaps")
-    r = int(round(rr ** 0.5))
+    rh, rw = _map_grid(rr, hw, "cross_heatmaps")
     arr = (C.c_void_p * len(maps))(*[m.data_ptr() for m in maps])
-    out = torch.empty((Fm, ntok, r, r), dtype=torch.uint8, device=m0.device)
-    _lib.call("fz_cross_heatmaps", arr, len(maps), int(m0.dtype == torch.float32), Fm, heads, r, m0.stride(2), int(ntok), _p(out), _stream())
+    out = torch.empty((Fm, ntok, rh, rw), dtype=torch.uint8, device=m0.device)
+    _lib.call("fz_cross_heatmaps_hw", arr, len(maps), int(m0.dtype == torch.float32), Fm, heads, rh, rw, m0.stride(2), int(ntok), _p(out),
+              _stream())
     return out
 
 

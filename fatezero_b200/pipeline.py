@@ -279,6 +279,13 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         if (callback_steps is None) or (callback_steps is not None and (not isinstance(callback_steps, int) or callback_steps <= 0)):
             raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps} of type {type(callback_steps)}.")
 
+    @staticmethod
+    def check_frame_size(height: int, width: int, where: str):
+        """A non-square clip must be a multiple of 64 pixels on both sides, so that the UNet's three stride-2 downsamples are exact and
+        every level holds (h >> k) x (w >> k) latents; square clips keep the multiple-of-8 rule of check_inputs."""
+        if height != width and (height % 64 or width % 64):
+            raise ValueError(f"{where}: a non-square clip needs height and width that are multiples of 64, got {height} x {width}")
+
     # ---- scheduler tables (work with diffusers' DDIMScheduler or fatezero_b200.scheduler.DDIMScheduler) -------------
     def _alpha(self, t: int) -> float:
         return float(self.scheduler.alphas_cumprod[int(t)]) if int(t) >= 0 else float(self.scheduler.final_alpha_cumprod)
@@ -288,6 +295,7 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
     def prepare_latents_ddim_inverted(self, image, batch_size, num_images_per_prompt, text_embeddings, store_attention=False,
                                       prompt=None, generator=None, LOW_RESOURCE=True, save_path=None):
         """p2p_ddim_spatial_temporal.py:68-129."""
+        self.check_frame_size(image.shape[-2], image.shape[-1], "prepare_latents_ddim_inverted")
         self.prepare_before_train_loop()
         if store_attention:
             attention_util.register_attention_control(self, self.store_controller)
@@ -545,6 +553,10 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         if len(set(geo)) != 1:
             raise ValueError(f"prepare_latents_ddim_inverted_batch: the clips differ in (frames, h, w): {geo}; batch clips of one geometry")
         F, h, w = geo[0]
+        if images is not None:
+            self.check_frame_size(clips[0].shape[2], clips[0].shape[3], "prepare_latents_ddim_inverted_batch")
+        else:
+            self.check_frame_size(h * self.vae_scale_factor, w * self.vae_scale_factor, "prepare_latents_ddim_inverted_batch")
         if K * F > self.MAX_BATCH_ROWS:
             raise ValueError(f"prepare_latents_ddim_inverted_batch: {K} clips x {F} frames = {K * F} rows exceed {self.MAX_BATCH_ROWS}")
         if self._engine_is_sharded():
@@ -613,6 +625,7 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         if len(set(shapes)) != 1:
             raise ValueError(f"p2preplace_edit_clips: the clips differ in shape {shapes}; batch clips of one (frames, h, w)")
         F = shapes[0][2]
+        self.check_frame_size(shapes[0][3] * self.vae_scale_factor, shapes[0][4] * self.vae_scale_factor, "p2preplace_edit_clips")
         if 2 * J * F > self.MAX_BATCH_ROWS:
             raise ValueError(f"p2preplace_edit_clips: 2 x {J} jobs x {F} frames = {2 * J * F} CFG rows exceed {self.MAX_BATCH_ROWS}")
         for k, j in enumerate(jobs):
@@ -680,6 +693,9 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         height = height or self.unet.config.sample_size * self.vae_scale_factor
         width = width or self.unet.config.sample_size * self.vae_scale_factor
         self.check_inputs(prompt, height, width, callback_steps, strength)
+        self.check_frame_size(height, width, "sd_ddim_pipeline")
+        if latents is not None:  # the clip's size is that of its latents
+            self.check_frame_size(latents.shape[-2] * self.vae_scale_factor, latents.shape[-1] * self.vae_scale_factor, "sd_ddim_pipeline")
         if eta != 0.0:
             raise NotImplementedError("FateZero's DDIM path is deterministic (eta = 0)")
         batch_size = 1 if isinstance(prompt, str) else len(prompt)

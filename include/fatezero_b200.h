@@ -204,7 +204,11 @@ int fz_cfg_ddim_step_batched(float* x, const float* eps2, int K, long long n_ite
 int fz_cfg_ddim_step_multi(float* x, const float* eps2, int K, long long n_item, float guidance, float alpha_t, float alpha_prev,
                            const float* const* x_inv, const float* const* mask_a, const float* const* mask_b, const int* apply_blend,
                            long long fhw, fz_stream_t stream);
-/* blend mask from cached cross maps (spatial_blend.py:24-39,78-111); maps: HOST array of device pointers, word_w: HOST [ntok] */
+/* blend mask from cached cross maps (spatial_blend.py:24-39,78-111); maps: HOST array of device pointers [F, heads, rh*rw, ldm],
+ * word_w: HOST [ntok].  The rh x rw grid (rh * rw <= 1024) is max-pooled and resized to h x w with F.interpolate's nearest index per axis.
+ * fz_blend_mask is the square grid rh = rw = r. */
+int fz_blend_mask_hw(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int rh, int rw, int ldm, int ntok,
+                     const float* word_w, float th, int h, int w, float* out, fz_stream_t stream);
 int fz_blend_mask(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int r, int ldm, int ntok, const float* word_w,
                   float th, int h, int w, float* out, fz_stream_t stream);
 
@@ -219,9 +223,12 @@ int fz_gelu_f16(void* x, long long n, fz_stream_t stream);
 /* in-place row softmax x[r, :n] <- softmax(scale * x[r, :n]), fp32 math: the VAE's 512-wide single-head attention runs GEMM -> this -> GEMM */
 int fz_softmax_rows_f16(void* x, long long rows, int n, long long ld, float scale, fz_stream_t stream);
 
-/* show_cross_attention on the device (prompt_attention/visualization.py:14-72): out[f, tok, res*res] = 255 * a / max(a) with a = sum over the
- * given cross-attention maps ([F, heads, res*res, ldm] fp16 or fp32 running sums) and heads of the probability of text token tok (the means'
- * constant factors cancel).  The reference averages every stored map and copies the r16 cross maps to the host first. */
+/* show_cross_attention on the device (prompt_attention/visualization.py:14-72): out[f, tok, rh*rw] = 255 * a / max(a) with a = sum over the
+ * given cross-attention maps ([F, heads, rh*rw, ldm] fp16 or fp32 running sums, rh * rw <= 1024) and heads of the probability of text token
+ * tok (the means' constant factors cancel).  The reference averages every stored map and copies the r16 cross maps to the host first.
+ * fz_cross_heatmaps is the square grid rh = rw = res. */
+int fz_cross_heatmaps_hw(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int rh, int rw, int ldm, int ntok,
+                         unsigned char* out, fz_stream_t stream);
 int fz_cross_heatmaps(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int res, int ldm, int ntok, unsigned char* out,
                       fz_stream_t stream);
 
