@@ -102,6 +102,7 @@ SIGNATURES = {
                                  C.POINTER(c_void_p), C.POINTER(c_int), c_ll, c_void_p],
     "fz_cfg_ddim_step_multi": [c_void_p, c_void_p, c_int, c_ll, c_float, c_float, c_float, C.POINTER(c_void_p), C.POINTER(c_void_p),
                                C.POINTER(c_void_p), C.POINTER(c_int), c_ll, c_void_p],
+    "fz_ddim_sample_step": [c_void_p, c_void_p, c_int, c_ll, c_int, c_float, c_float, c_float, c_float, c_void_p, c_void_p],
     "fz_blend_mask": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(c_float), c_float, c_int, c_int,
                       c_void_p, c_void_p],
     "fz_blend_mask_hw": [C.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(c_float), c_float, c_int,

@@ -700,6 +700,45 @@ __global__ void cfg_ddim_kernel(float* __restrict__ x, const float* __restrict__
   }
 }
 
+// One DDIM sampling step of diffusers' DDIMScheduler.step (eta >= 0) after the guidance of stable_diffusion.py:533-541, on K items of
+// n_item elements: x [K, n_item]; eps = [uncond_1..K | cond_1..K] (cfg = 1) or [K, n_item] (cfg = 0); noise [K, n_item] or null when
+// sigma = 0.  The guidance, x0 and direction terms are written as in cfg_ddim_kernel, so cfg = 1, sigma = 0 is bitwise that kernel without
+// blend.  V = 4 moves float4 vectors (every pointer 16-byte aligned, K * n_item a multiple of 4), V = 1 single elements.
+template <int V>
+__global__ void ddim_sample_kernel(float* __restrict__ x, const float* __restrict__ eps, long long n, int cfg, float guidance, float sqrt_a_t,
+                                   float sqrt_1m_a_t, float sqrt_a_prev, float dir, float sigma, const float* __restrict__ noise) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long nv = n / V;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nv; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float xv[V], eu[V], ec[V], z[V];
+    if constexpr (V == 4) {
+      *reinterpret_cast<float4*>(xv) = reinterpret_cast<const float4*>(x)[i];
+      *reinterpret_cast<float4*>(eu) = reinterpret_cast<const float4*>(eps)[i];
+      if (cfg) *reinterpret_cast<float4*>(ec) = reinterpret_cast<const float4*>(eps + n)[i];
+      if (noise) *reinterpret_cast<float4*>(z) = reinterpret_cast<const float4*>(noise)[i];
+    } else {
+      xv[0] = x[i];
+      eu[0] = eps[i];
+      if (cfg) ec[0] = eps[n + i];
+      if (noise) z[0] = noise[i];
+    }
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+      const float e = cfg ? eu[j] + guidance * (ec[j] - eu[j]) : eu[j];
+      const float x0 = (xv[j] - sqrt_1m_a_t * e) / sqrt_a_t;
+      float xn = sqrt_a_prev * x0 + dir * e;
+      if (noise) xn = xn + sigma * z[j];
+      xv[j] = xn;
+    }
+    if constexpr (V == 4) {
+      reinterpret_cast<float4*>(x)[i] = *reinterpret_cast<const float4*>(xv);
+    } else {
+      x[i] = xv[0];
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Blend mask (spatial_blend.py:24-39, 78-111): mean over (layers, heads) of sum_n map[f,hd,p,n]*w[n] on the rh x rw grid,
 // 3x3 max-pool (stride 1, pad 1), nearest resize to (h, w), divide by the per-frame max, compare with th.
@@ -1059,6 +1098,26 @@ extern "C" int fz_cfg_ddim_step_multi(float* x, const float* eps2, int K, long l
                  k);
   }
   return cfg_ddim_launch(x, eps2, K, n_item, guidance, a_t, a_prev, items, fhw, stream);
+}
+
+extern "C" int fz_ddim_sample_step(float* x, const float* eps, int K, long long n_item, int cfg, float guidance, float a_t, float a_prev,
+                                   float sigma, const float* noise, cudaStream_t stream) {
+  FZ_CHECK_ARG(x && eps && K >= 1 && n_item > 0, "fz_ddim_sample_step: null pointer or empty batch");
+  FZ_CHECK_ARG(sigma >= 0.f && (sigma == 0.f || noise), "fz_ddim_sample_step: sigma=%g needs noise", static_cast<double>(sigma));
+  const long long n = static_cast<long long>(K) * n_item;
+  if (sigma == 0.f) noise = nullptr;
+  const float sqrt_a_t = sqrtf(a_t), sqrt_1m_a_t = sqrtf(1.f - a_t), sqrt_a_prev = sqrtf(a_prev);
+  const float dir = sqrtf(1.f - a_prev - sigma * sigma);
+  auto aligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  if (n % 4 == 0 && aligned(x) && aligned(eps) && (!noise || aligned(noise))) {
+    FZ_CUDA(launch_pdl(ddim_sample_kernel<4>, dim3(grid_for(n / 4, 256)), dim3(256), 0, stream, x, eps, n, cfg, guidance, sqrt_a_t,
+                       sqrt_1m_a_t, sqrt_a_prev, dir, sigma, noise));
+  } else {
+    FZ_CUDA(launch_pdl(ddim_sample_kernel<1>, dim3(grid_for(n, 256)), dim3(256), 0, stream, x, eps, n, cfg, guidance, sqrt_a_t, sqrt_1m_a_t,
+                       sqrt_a_prev, dir, sigma, noise));
+  }
+  FZ_CUDA(cudaGetLastError());
+  return FZ_OK;
 }
 
 extern "C" int fz_blend_mask_hw(const void* const* maps, int num_maps, int maps_f32, int F, int heads, int rh, int rw, int ldm, int ntok,

@@ -474,8 +474,10 @@ class UNetEngine:
 
     # ---------------------------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def forward(self, x: torch.Tensor, t: float, text: torch.Tensor, ctrl=None) -> torch.Tensor:
-        """x [B,4,F,H,W] (any float dtype, CUDA), text [B,77,D] -> eps [B,4,F,H,W] fp32."""
+    def forward(self, x: torch.Tensor, t: float, text: torch.Tensor, ctrl=None, items: int = 1) -> torch.Tensor:
+        """x [B,4,F,H,W] (any float dtype, CUDA), text [B,77,D] -> eps [B,4,F,H,W] fp32.
+        items (controller-free batches of several clips): the batch holds `items` equal-sized items, and the GroupNorm chunking is planned
+        per item so that every clip's statistics are bitwise those of a batch of its item alone (as controller.prompt_groups does)."""
         self._foreign = None
         if ctrl is not None and not hasattr(ctrl, "self_attn_args"):
             if type(ctrl).__name__ in ("EmptyControl", "DummyController"):
@@ -492,7 +494,7 @@ class UNetEngine:
         if text.shape[0] != B:
             raise ValueError(f"encoder_hidden_states batch {text.shape[0]} != sample batch {B}")
         self._ensure_text(text)
-        groups = getattr(ctrl, "prompt_groups", 1) if ctrl is not None else 1
+        groups = getattr(ctrl, "prompt_groups", 1) if ctrl is not None else int(items)
         if groups > 1 and self.shard is not None:
             raise NotImplementedError("a batched multi-prompt edit does not run frame-sharded")
         if groups > 1 and B % groups:

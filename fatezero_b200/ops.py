@@ -290,6 +290,24 @@ def cfg_ddim_step_multi(x: torch.Tensor, eps2: torch.Tensor, guidance: float, a_
               _stream())
 
 
+def ddim_sample_step(x: torch.Tensor, eps: torch.Tensor, guidance: Optional[float], a_t: float, a_prev: float, sigma: float = 0.0,
+                     noise: Optional[torch.Tensor] = None):
+    """x [K, 4, F, h, w] fp32 (K clips) <- one DDIM sampling step.  guidance=None: eps [K, ...] is the noise prediction itself; otherwise
+    eps [2K, ...] = [uncond_1..K ; cond_1..K] is guided with it.  sigma > 0 needs noise [K, ...] fp32."""
+    K = x.shape[0]
+    _chk(x, torch.float32, "ddim_sample_step")
+    _chk(eps, torch.float32, "ddim_sample_step")
+    cfg = guidance is not None
+    if eps.numel() != (2 if cfg else 1) * x.numel() or not (x.is_contiguous() and eps.is_contiguous()):
+        raise ValueError(f"ddim_sample_step: eps {tuple(eps.shape)} does not match x {tuple(x.shape)} (cfg={cfg}) or is not contiguous")
+    if sigma > 0:
+        if noise is None or noise.numel() != x.numel() or not noise.is_contiguous():
+            raise ValueError("ddim_sample_step: sigma > 0 needs contiguous noise shaped like x")
+        _chk(noise, torch.float32, "ddim_sample_step")
+    _lib.call("fz_ddim_sample_step", _p(x), _p(eps), K, x.numel() // K, int(cfg), float(guidance or 0.0), float(a_t), float(a_prev),
+              float(sigma), _p(noise) if sigma > 0 else None, _stream())
+
+
 def _same_map_geometry(maps: Sequence[torch.Tensor], what: str):
     """The map kernels read every map with the first one's [F, heads, r*r] and row stride and average over maps x heads: a map of another
     head count (SD-2.x stores 5 / 10 / 20 heads at different levels) would be misread and misweighted."""

@@ -5,6 +5,9 @@ P2pSampleLogger (pipelines/p2p_validation_loop.py) drive it unchanged.
 The two hot loops run on the GPU through libfatezero_b200.so:
   ddim_clean2noisy_loop  : N x { UNet (B=1, STORE fused in attention) ; fz_ddim_invert_step }
   sd_ddim_pipeline loop  : N x { UNet (B=2, INJECT/BLEND fused)       ; fz_cfg_ddim_step (+ latent blend) }
+  _sample_loop           : N x { UNet (whole clips, un-hooked)       ; fz_ddim_sample_step (CFG or not, eta >= 0) }
+The last one serves text-to-video sampling (SpatioTemporalStableDiffusionPipeline.__call__, pipelines/stable_diffusion.py:403-564) and the
+Tune-A-Video + DDIM inversion baseline (DDIMSpatioTemporalStableDiffusionPipeline, pipelines/ddim_spatial_temporal.py).
 Latents stay fp32 in HBM for the whole run; text encoder / VAE / tokenizer are whatever objects the caller passes (out of the
 accelerated scope, SURVEY.md §8(f)).
 """
@@ -64,6 +67,16 @@ class SpatioTemporalStableDiffusionPipeline:
                         dict(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler).items()}
         self.vae_scale_factor = 2 ** (len(self.vae.config.block_out_channels) - 1)
         self._progress_bar_config = {}
+        # CUDA-graph execution of the DDIM loops (graphs.py): "auto" = eager the first time a configuration is seen, captured and
+        # replayed from its second occurrence on; "off" = always eager
+        self.graph_mode = os.environ.get("FZ_GRAPHS", "auto")
+        self._plans = {}
+        self._seen = set()
+
+    def release_graphs(self):
+        """Drop every captured plan (and the HBM pools that hold their map caches)."""
+        self._plans.clear()
+        self._seen.clear()
 
     # ---- DiffusionPipeline surface ------------------------------------------------------------------------------
     @property
@@ -253,22 +266,6 @@ class SpatioTemporalStableDiffusionPipeline:
         return out
 
 
-class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
-    def __init__(self, vae, text_encoder, tokenizer, unet, scheduler, disk_store: bool = False):
-        super().__init__(vae, text_encoder, tokenizer, unet, scheduler)
-        self.store_controller = attention_util.AttentionStore(disk_store=disk_store)
-        self.empty_controller = attention_util.EmptyControl()
-        # CUDA-graph execution of the two DDIM loops (graphs.py): "auto" = eager the first time a configuration is seen, captured and
-        # replayed from its second occurrence on; "off" = always eager
-        self.graph_mode = os.environ.get("FZ_GRAPHS", "auto")
-        self._plans = {}
-        self._seen = set()
-
-    def release_graphs(self):
-        """Drop every captured plan (and the HBM pools that hold their map caches)."""
-        self._plans.clear()
-        self._seen.clear()
-
     def check_inputs(self, prompt, height, width, callback_steps, strength=None):
         if not isinstance(prompt, str) and not isinstance(prompt, list):
             raise ValueError(f"`prompt` has to be of type `str` or `list` but is {type(prompt)}")
@@ -286,22 +283,18 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         if height != width and (height % 64 or width % 64):
             raise ValueError(f"{where}: a non-square clip needs height and width that are multiples of 64, got {height} x {width}")
 
+    def _engine_is_sharded(self) -> bool:
+        engine = getattr(self.unet, "_engine", None)  # not built here: nothing may touch the GPU before the checks pass
+        return getattr(engine, "shard", None) is not None
+
     # ---- scheduler tables (work with diffusers' DDIMScheduler or fatezero_b200.scheduler.DDIMScheduler) -------------
     def _alpha(self, t: int) -> float:
         return float(self.scheduler.alphas_cumprod[int(t)]) if int(t) >= 0 else float(self.scheduler.final_alpha_cumprod)
 
-    # ---- inversion ----------------------------------------------------------------------------------------------------
-    @torch.no_grad()
-    def prepare_latents_ddim_inverted(self, image, batch_size, num_images_per_prompt, text_embeddings, store_attention=False,
-                                      prompt=None, generator=None, LOW_RESOURCE=True, save_path=None):
-        """p2p_ddim_spatial_temporal.py:68-129."""
-        self.check_frame_size(image.shape[-2], image.shape[-1], "prepare_latents_ddim_inverted")
-        self.prepare_before_train_loop()
-        if store_attention:
-            attention_util.register_attention_control(self, self.store_controller)
-        resource_default_value = self.store_controller.LOW_RESOURCE
-        self.store_controller.LOW_RESOURCE = LOW_RESOURCE
-        batch_size = batch_size * num_images_per_prompt
+    # ---- DDIM inversion (p2p_ddim_spatial_temporal.py:68-161, ddim_spatial_temporal.py:45-119) -------------------------
+    def _clean_latents_bcfhw(self, image, batch_size, generator):
+        """VAE-encode the frames `image` [(b f), 3, H, W] and split them into `batch_size` clips [b, 4, f, h, w] (duplicating the clip when
+        fewer images than clips are given)."""
         if isinstance(generator, list) and len(generator) != batch_size:
             raise ValueError(f"You have passed a list of generators of length {len(generator)}, but requested an effective batch size of "
                              f"{batch_size}. Make sure the batch size matches the length of the generators.")
@@ -315,15 +308,7 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         if batch_size > init_latents.shape[0]:
             init_latents = torch.cat([init_latents] * (batch_size // init_latents.shape[0]), dim=0)
         bf, c, h, w = init_latents.shape
-        init_bcfhw = init_latents.reshape(batch_size, bf // batch_size, c, h, w).permute(0, 2, 1, 3, 4)
-        out = self.ddim_clean2noisy_loop(init_bcfhw, text_embeddings, self.store_controller)
-        if store_attention and (save_path is not None):
-            os.makedirs(save_path + "/cross_attention")
-            from .visualization import show_cross_attention
-            show_cross_attention(self.tokenizer, prompt, self.store_controller, 16, ["up", "down"], save_path=save_path + "/cross_attention")
-            attention_util.register_attention_control(self, self.empty_controller)
-        self.store_controller.LOW_RESOURCE = resource_default_value
-        return out
+        return init_latents.reshape(batch_size, bf // batch_size, c, h, w).permute(0, 2, 1, 3, 4)
 
     @torch.no_grad()
     def ddim_clean2noisy_loop(self, latent, text_embeddings, controller=None, teacher_latents=None):
@@ -398,6 +383,195 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
         t_start = max(num_inference_steps - init_timestep, 0)
         return self.scheduler.timesteps[t_start:], num_inference_steps - t_start
+
+    # ---- text-to-video sampling (stable_diffusion.py:355-564) -----------------------------------------------------------
+    MAX_SAMPLE_ROWS = 64  # attention rows (CFG halves x clips x frames) of one un-hooked UNet call: kMaxBF of fz_attention_f16
+
+    def prepare_latents(self, batch_size, num_channels_latents, clip_length, height, width, dtype, device, generator, latents=None):
+        """stable_diffusion.py:355-401: Gaussian latents [batch_size, C, clip_length, h, w] (one draw per generator of a list)."""
+        shape = (batch_size, num_channels_latents, clip_length, height // self.vae_scale_factor, width // self.vae_scale_factor)
+        if isinstance(generator, list) and len(generator) != batch_size:
+            raise ValueError(f"You have passed a list of generators of length {len(generator)}, but requested an effective batch size of "
+                             f"{batch_size}. Make sure the batch size matches the length of the generators.")
+        if latents is None:
+            if isinstance(generator, list):
+                latents = torch.cat([torch.randn((1,) + shape[1:], generator=g, device=device, dtype=dtype) for g in generator]).to(device)
+            else:
+                latents = torch.randn(shape, generator=generator, device=device, dtype=dtype).to(device)
+        else:
+            if latents.shape != shape:
+                raise ValueError(f"Unexpected latents shape, got {latents.shape}, expected {shape}")
+            latents = latents.to(device)
+        return latents * self.scheduler.init_noise_sigma
+
+    def _check_sampling(self, guidance_scale, eta, generator, clip_length):
+        """The refusals of the sampler, before any GPU work."""
+        if eta < 0:
+            raise ValueError(f"eta must be >= 0, got {eta}")
+        if eta > 0 and isinstance(generator, list):
+            # DDIMScheduler.step draws its noise with torch.randn(generator=generator), which takes one generator
+            raise ValueError("eta > 0 draws each step's noise from one generator: a list of generators is not supported")
+        if self._engine_is_sharded():
+            raise NotImplementedError("text-to-video sampling does not run frame-sharded")
+        rows = (2 if guidance_scale > 1.0 else 1) * clip_length
+        if rows > self.MAX_SAMPLE_ROWS:
+            raise ValueError(f"a clip of {clip_length} frames needs {rows} attention rows per UNet call (CFG doubles them), more than "
+                             f"{self.MAX_SAMPLE_ROWS}")
+
+    def _ddim_sigma(self, t: int, eta: float) -> float:
+        """eta * sqrt(DDIMScheduler._get_variance(t, t_prev)) of diffusers 0.11.1."""
+        a_t, a_p = self._alpha(t), self._alpha(t - self.scheduler.config.num_train_timesteps // self.scheduler.num_inference_steps)
+        return float(eta) * (((1 - a_p) / (1 - a_t)) * (1 - a_t / a_p)) ** 0.5
+
+    def _sample_loop(self, latents, text_embeddings, guidance_scale, eta, generator, callback, callback_steps, variance_noise=None,
+                     teacher_latents=None):
+        """The denoising loop of stable_diffusion.py:519-549 (also ddim_spatial_temporal.py:255-284) on the un-hooked sm_90a UNet and
+        fz_ddim_sample_step.  Clips run together in UNet calls of at most MAX_SAMPLE_ROWS attention rows; every clip gets, bit for bit, what
+        a call of that clip alone gives it.  At eta > 0, step i adds sigma_i * z_i with z_i = torch.randn of the guided noise's shape from
+        `generator` (the draw of DDIMScheduler.step), drawn in step order.  Returns the final latents in the latents' dtype.
+        variance_noise / teacher_latents (parity tests only): the per-step noise to use instead of drawing it, and the reference latents
+        after each step (step i > 0 then starts from teacher_latents[i - 1])."""
+        latents_dtype = latents.dtype
+        dev = self.unet.device
+        engine = self.unet.engine()
+        do_cfg = guidance_scale > 1.0
+        timesteps = [int(t) for t in self.scheduler.timesteps]
+        n = len(timesteps)
+        step = self.scheduler.config.num_train_timesteps // self.scheduler.num_inference_steps
+        coef = [(self._alpha(t), self._alpha(t - step), self._ddim_sigma(t, eta)) for t in timesteps]
+        stochastic = eta > 0
+        B, F = latents.shape[0], latents.shape[2]
+        per_call = max(1, self.MAX_SAMPLE_ROWS // ((2 if do_cfg else 1) * F))
+        spans = [(a, min(B, a + per_call)) for a in range(0, B, per_call)]
+        text = text_embeddings.to(dev)
+        if do_cfg:
+            uncond, cond = text.chunk(2)
+            texts = [torch.cat([uncond[a:b], cond[a:b]]).contiguous() for a, b in spans]
+        else:
+            texts = [text[a:b].contiguous() for a, b in spans]
+
+        def draw(i):
+            if variance_noise is not None:
+                return variance_noise[i].to(dev, torch.float32)
+            return torch.randn(latents.shape, generator=generator, device=dev, dtype=latents_dtype).to(torch.float32)
+
+        def sample_step(i, x, texts_, z):
+            t = timesteps[i]
+            a_t, a_p, sigma = coef[i]
+            for (a, b), tx in zip(spans, texts_):
+                xc = x[a:b]
+                eps = engine.forward(torch.cat([xc, xc]) if do_cfg else xc, float(t), tx, None, items=b - a)
+                ops.ddim_sample_step(xc, eps, guidance_scale if do_cfg else None, a_t, a_p, sigma, None if z is None else z[a:b])
+
+        with torch.cuda.device(dev):
+            key = None
+            if self.graph_mode != "off" and teacher_latents is None:
+                key = ("sample", tuple(latents.shape), tuple(timesteps), tuple(text.shape), float(guidance_scale), float(eta), id(engine),
+                       engine.shard_signature())
+            if key is not None and (key in self._plans or key in self._seen):
+                plan = self._plans.get(key)
+                if plan is None:
+                    from .graphs import LoopPlan
+                    plan = LoopPlan(dev)
+                    plan.x = torch.empty(latents.shape, dtype=torch.float32, device=dev)
+                    plan.text = [torch.empty_like(tx) for tx in texts]
+                    plan.noise = torch.zeros((n, *latents.shape), dtype=torch.float32, device=dev) if stochastic else None
+                    plan.x.copy_(latents)
+                    for buf, tx in zip(plan.text, texts):
+                        buf.copy_(tx)
+                    for i in range(n):
+                        plan.steps.capture(lambda i=i: sample_step(i, plan.x, plan.text, None if plan.noise is None else plan.noise[i]))
+                    self._plans[key] = plan
+                # every step's noise is drawn before the replay, one draw per step in step order: the generator advances as in the eager loop
+                if stochastic:
+                    for i in range(n):
+                        plan.noise[i].copy_(draw(i))
+                plan.x.copy_(latents)
+                for buf, tx in zip(plan.text, texts):
+                    buf.copy_(tx)
+                for i in range(n):
+                    plan.steps.replay(i)
+                    if callback is not None and i % callback_steps == 0:
+                        callback(i, timesteps[i], plan.x.to(latents_dtype))
+                x = plan.x.clone()
+            else:
+                if key is not None:
+                    self._seen.add(key)
+                x = latents.detach().to(dev, torch.float32).contiguous().clone()
+                for i, t in enumerate(timesteps):
+                    if teacher_latents is not None and i > 0:
+                        x.copy_(teacher_latents[i - 1].to(dev, torch.float32))
+                    sample_step(i, x, texts, draw(i) if stochastic else None)
+                    if callback is not None and i % callback_steps == 0:
+                        callback(i, t, x.to(latents_dtype))
+        return x.to(latents_dtype)
+
+    def _sample_output(self, latents, output_type, return_dict):
+        if output_type == "latent":
+            image = latents
+        else:
+            image = self.decode_latents(latents)
+            if output_type == "pil":
+                image = self.numpy_to_pil(image)
+        if not return_dict:
+            return (image, None)
+        return StableDiffusionPipelineOutput(images=image, nsfw_content_detected=None)
+
+    @torch.no_grad()
+    def __call__(self, prompt: Union[str, List[str]], height: Optional[int] = None, width: Optional[int] = None, num_inference_steps: int = 50,
+                 clip_length: int = 8, guidance_scale: float = 7.5, negative_prompt: Optional[Union[str, List[str]]] = None,
+                 num_images_per_prompt: Optional[int] = 1, eta: float = 0.0,
+                 generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None, latents: Optional[torch.FloatTensor] = None,
+                 output_type: Optional[str] = "pil", return_dict: bool = True,
+                 callback: Optional[Callable[[int, int, torch.FloatTensor], None]] = None, callback_steps: Optional[int] = 1,
+                 variance_noise=None, teacher_latents=None):
+        """Text-to-video generation, stable_diffusion.py:403-564: Gaussian latents (prepare_latents), then `num_inference_steps` DDIM steps
+        with classifier-free guidance when guidance_scale > 1 and the stochastic DDIM noise of eta > 0 (diffusers' DDIMScheduler.step).
+        The DDIM arithmetic runs in fp32 on the GPU.  output_type: "pil", "numpy" or "latent".
+        variance_noise / teacher_latents are for parity tests only (see _sample_loop)."""
+        height = height or self.unet.config.sample_size * self.vae_scale_factor
+        width = width or self.unet.config.sample_size * self.vae_scale_factor
+        self.check_inputs(prompt, height, width, callback_steps)
+        self.check_frame_size(height, width, "__call__")
+        self._check_sampling(guidance_scale, eta, generator, clip_length)
+        batch_size = 1 if isinstance(prompt, str) else len(prompt)
+        device = self._execution_device
+        do_cfg = guidance_scale > 1.0
+        text_embeddings = self._encode_prompt(prompt, device, num_images_per_prompt, do_cfg, negative_prompt)
+        self.scheduler.set_timesteps(num_inference_steps, device=device)
+        latents = self.prepare_latents(batch_size * num_images_per_prompt, self.unet.config.in_channels, clip_length, height, width,
+                                       text_embeddings.dtype, device, generator, latents)
+        latents = self._sample_loop(latents, text_embeddings, guidance_scale, eta, generator, callback, callback_steps, variance_noise,
+                                    teacher_latents)
+        return self._sample_output(latents, output_type, return_dict)
+
+
+class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
+    def __init__(self, vae, text_encoder, tokenizer, unet, scheduler, disk_store: bool = False):
+        super().__init__(vae, text_encoder, tokenizer, unet, scheduler)
+        self.store_controller = attention_util.AttentionStore(disk_store=disk_store)
+        self.empty_controller = attention_util.EmptyControl()
+
+    # ---- inversion ----------------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def prepare_latents_ddim_inverted(self, image, batch_size, num_images_per_prompt, text_embeddings, store_attention=False,
+                                      prompt=None, generator=None, LOW_RESOURCE=True, save_path=None):
+        """p2p_ddim_spatial_temporal.py:68-129."""
+        self.check_frame_size(image.shape[-2], image.shape[-1], "prepare_latents_ddim_inverted")
+        self.prepare_before_train_loop()
+        if store_attention:
+            attention_util.register_attention_control(self, self.store_controller)
+        resource_default_value = self.store_controller.LOW_RESOURCE
+        self.store_controller.LOW_RESOURCE = LOW_RESOURCE
+        init_bcfhw = self._clean_latents_bcfhw(image, batch_size * num_images_per_prompt, generator)
+        out = self.ddim_clean2noisy_loop(init_bcfhw, text_embeddings, self.store_controller)
+        if store_attention and (save_path is not None):
+            os.makedirs(save_path + "/cross_attention")
+            from .visualization import show_cross_attention
+            show_cross_attention(self.tokenizer, prompt, self.store_controller, 16, ["up", "down"], save_path=save_path + "/cross_attention")
+            attention_util.register_attention_control(self, self.empty_controller)
+        self.store_controller.LOW_RESOURCE = resource_default_value
+        return out
 
     # ---- edit -----------------------------------------------------------------------------------------------------------
     def _make_edit_controller(self, prompt: str, source_prompt: str, num_inference_steps: int, store=None, **kwargs):
@@ -501,10 +675,6 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         return results
 
     # ---- several source clips in one pass (test_fatezero_dataset.py sweeps clip after clip) --------------------------------------
-    def _engine_is_sharded(self) -> bool:
-        engine = getattr(self.unet, "_engine", None)  # not built here: nothing may touch the GPU before the checks pass
-        return getattr(engine, "shard", None) is not None
-
     def map_cache_admission(self, clips: int, frames: int, h: int, w: int, steps: int, save_self_attention: bool = True,
                             free_bytes: Optional[int] = None) -> int:
         """Bytes of the inversion map caches of `clips` clips of `frames` frames at latent size h x w over `steps` DDIM steps (the slab
@@ -823,3 +993,54 @@ class P2pDDIMSpatioTemporalPipeline(SpatioTemporalStableDiffusionPipeline):
         print(torch.tensor(1.0).cuda() * 2)
         from . import _lib
         print(f"libfatezero_b200 version {_lib.load().fz_version()} at {_lib.LIB_PATH}")
+
+
+class DDIMSpatioTemporalStableDiffusionPipeline(SpatioTemporalStableDiffusionPipeline):
+    """Drop-in for video_diffusion/pipelines/ddim_spatial_temporal.py (the "Tune-A-Video + DDIM inversion" baseline): DDIM-invert the
+    clip with the source prompt, then denoise it with the target prompt under classifier-free guidance, with no attention control.  The
+    inversion is the shared ddim_clean2noisy_loop, the denoising the text-to-video sampler's loop (_sample_loop)."""
+
+    @torch.no_grad()
+    def prepare_latents_ddim_inverted(self, image, batch_size, num_images_per_prompt, text_embeddings, generator=None):
+        """ddim_spatial_temporal.py:45-90: VAE-encode `image` [(b f), 3, H, W] with b = batch_size * num_images_per_prompt, invert it with
+        the cond half of `text_embeddings` ([uncond ; cond]) and return the N+1 latents ([0] clean, [-1] x_T)."""
+        self.check_frame_size(image.shape[-2], image.shape[-1], "prepare_latents_ddim_inverted")
+        init_bcfhw = self._clean_latents_bcfhw(image, batch_size * num_images_per_prompt, generator)
+        return self.ddim_clean2noisy_loop(init_bcfhw, text_embeddings)
+
+    @torch.no_grad()
+    def __call__(self, prompt: Union[str, List[str]], image=None, height: Optional[int] = None, width: Optional[int] = None,
+                 strength: float = None, num_inference_steps: int = 50, clip_length: int = 8, guidance_scale: float = 7.5,
+                 negative_prompt: Optional[Union[str, List[str]]] = None, num_images_per_prompt: Optional[int] = 1, eta: float = 0.0,
+                 generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None, latents: Optional[torch.FloatTensor] = None,
+                 output_type: Optional[str] = "pil", return_dict: bool = True,
+                 callback: Optional[Callable[[int, int, torch.FloatTensor], None]] = None, callback_steps: Optional[int] = 1, **args):
+        """ddim_spatial_temporal.py:130-299.  Without `latents` the clip `image` is inverted first (prepare_latents_ddim_inverted) with
+        the prompt's own embeddings, which needs guidance_scale > 1 ([uncond ; cond]).  `strength` is validated and otherwise unused, and the
+        keys SampleLogger passes (edit_type, source_prompt, uncond_embeddings_list, ...) are swallowed, as in the reference.  The parity-test
+        hooks variance_noise / teacher_latents of _sample_loop are read from those keys."""
+        height = height or self.unet.config.sample_size * self.vae_scale_factor
+        width = width or self.unet.config.sample_size * self.vae_scale_factor
+        self.check_inputs(prompt, height, width, callback_steps, strength)
+        batch_size = 1 if isinstance(prompt, str) else len(prompt)
+        do_cfg = guidance_scale > 1.0
+        if latents is not None:
+            self.check_frame_size(latents.shape[-2] * self.vae_scale_factor, latents.shape[-1] * self.vae_scale_factor, "__call__")
+            frames = latents.shape[2]
+        else:
+            if image is None:
+                raise ValueError("pass the clip to invert (`image`) or its inverted `latents`")
+            if not do_cfg:
+                # the inversion reads the cond half of [uncond ; cond] (ddim_spatial_temporal.py:95): there is none without guidance
+                raise ValueError("inverting the clip needs guidance_scale > 1 (the [uncond ; cond] text embeddings)")
+            self.check_frame_size(image.shape[-2], image.shape[-1], "__call__")
+            frames = image.shape[0] // (batch_size * num_images_per_prompt)
+        self._check_sampling(guidance_scale, eta, generator, frames)
+        device = self._execution_device
+        text_embeddings = self._encode_prompt(prompt, device, num_images_per_prompt, do_cfg, negative_prompt)
+        self.scheduler.set_timesteps(num_inference_steps, device=device)
+        if latents is None:
+            latents = self.prepare_latents_ddim_inverted(image, batch_size, num_images_per_prompt, text_embeddings, generator)[-1]
+        latents = self._sample_loop(latents, text_embeddings, guidance_scale, eta, generator, callback, callback_steps,
+                                    args.get("variance_noise"), args.get("teacher_latents"))
+        return self._sample_output(latents, output_type, return_dict)

@@ -61,14 +61,27 @@ class DDIMScheduler:
         a_p = float(self.alphas_cumprod[prev]) if prev >= 0 else float(self.final_alpha_cumprod)
         return a_t, a_p
 
+    def sigma(self, timestep: int, eta: float) -> float:
+        """eta * sqrt(_get_variance) of diffusers-0.11.1 DDIMScheduler: the standard deviation of the noise a step adds."""
+        a_t, a_p = self.alpha_pair(timestep)
+        return float(eta) * (((1 - a_p) / (1 - a_t)) * (1 - a_t / a_p)) ** 0.5
+
     def step(self, model_output, timestep, sample, eta: float = 0.0, use_clipped_model_output=False, generator=None,
              variance_noise=None, return_dict: bool = True):
-        """Torch-tensor API kept for callers outside the fused loop (deterministic eta=0 path)."""
-        if eta != 0.0:
-            raise NotImplementedError("FateZero edits with eta=0 (p2p_ddim_spatial_temporal.py:272)")
+        """Torch-tensor API for callers outside the fused loops, with diffusers-0.11.1 semantics: at eta > 0 the step adds
+        sigma * variance_noise, drawn as torch.randn(model_output.shape, generator=generator) on model_output's device and dtype when not
+        given (giving both is a ValueError), and the direction term becomes sqrt(1 - a_prev - sigma^2) * model_output."""
         a_t, a_p = self.alpha_pair(timestep)
         x0 = (sample - (1 - a_t) ** 0.5 * model_output) / a_t ** 0.5
         if self.config.clip_sample:
             x0 = x0.clamp(-1, 1)
-        prev = a_p ** 0.5 * x0 + (1 - a_p) ** 0.5 * model_output
+        std = self.sigma(timestep, eta)
+        prev = a_p ** 0.5 * x0 + (1 - a_p - std ** 2) ** 0.5 * model_output
+        if eta > 0:
+            if variance_noise is not None and generator is not None:
+                raise ValueError("Cannot pass both generator and variance_noise. Please make sure that either `generator` or `variance_noise` "
+                                 "stays `None`.")
+            if variance_noise is None:
+                variance_noise = torch.randn(model_output.shape, generator=generator, device=model_output.device, dtype=model_output.dtype)
+            prev = prev + std * variance_noise
         return SimpleNamespace(prev_sample=prev, pred_original_sample=x0)

@@ -204,6 +204,13 @@ int fz_cfg_ddim_step_batched(float* x, const float* eps2, int K, long long n_ite
 int fz_cfg_ddim_step_multi(float* x, const float* eps2, int K, long long n_item, float guidance, float alpha_t, float alpha_prev,
                            const float* const* x_inv, const float* const* mask_a, const float* const* mask_b, const int* apply_blend,
                            long long fhw, fz_stream_t stream);
+/* x <- one DDIM sampling step (stable_diffusion.py:533-541 + diffusers-0.11.1 DDIMScheduler.step with eta) on K items of n_item fp32
+ * elements: e = eu + guidance (ec - eu) with eps = [uncond_1..K ; cond_1..K] (cfg = 1) or e = eps [K, n_item] (cfg = 0);
+ * x0 = (x - sqrt(1 - alpha_t) e) / sqrt(alpha_t); x <- sqrt(alpha_prev) x0 + sqrt(1 - alpha_prev - sigma^2) e + sigma noise.
+ * sigma = eta sqrt((1 - alpha_prev) / (1 - alpha_t)) sqrt(1 - alpha_t / alpha_prev) >= 0; noise [K, n_item] fp32 (NULL allowed when
+ * sigma = 0).  cfg = 1, sigma = 0 is bitwise fz_cfg_ddim_step without blend. */
+int fz_ddim_sample_step(float* x, const float* eps, int K, long long n_item, int cfg, float guidance, float alpha_t, float alpha_prev,
+                        float sigma, const float* noise, fz_stream_t stream);
 /* blend mask from cached cross maps (spatial_blend.py:24-39,78-111); maps: HOST array of device pointers [F, heads, rh*rw, ldm],
  * word_w: HOST [ntok].  The rh x rw grid (rh * rw <= 1024) is max-pooled and resized to h x w with F.interpolate's nearest index per axis.
  * fz_blend_mask is the square grid rh = rw = r. */
